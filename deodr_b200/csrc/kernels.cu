@@ -236,13 +236,33 @@ __global__ void k_publish(const int *scal, int *host_totals, int seq) {
 // Small triangles: the tile's pre-masked records are pulled into shared memory by bulk copies (cp.async.bulk +
 // mbarrier, SASS UBLKCP) 128 at a time through a two-deep pipeline - chunks c and c+1 are in flight when the tile
 // starts, chunk c+2 is issued as soon as chunk c has been consumed, so a crowded tile (the 1M-triangle scene has 400
-// tiles with more than 256 records, the 200k-triangle 512^2 views average 280) pays the copy latency once; two threads
-// per record scatter its index into per-pixel candidate lists; each pixel then z-tests its own candidates exactly.
+// tiles with more than 256 records, the 200k-triangle 512^2 views average 280) pays the copy latency once.  A chunk of
+// at most WARP_TEST_MAX records (most tiles of that scene: 62 records on average) is z-tested warp by warp: warp p
+// needs only mask word p of each record, so it finds its pixels' candidates by itself and no CTA barrier separates the
+// copy from the test.  A larger chunk has two threads per record scatter its index into per-pixel candidate lists,
+// then, after a barrier, each pixel z-tests its own candidates exactly.
 // Large triangles: stencil per triangle -> coverage masks (8 threads each) -> mask test.
 // One tile per CTA, scheduled by the hardware rather than persistent CTAs with a static stride: the tiles are very
 // uneven.
 #ifndef DEODR_TILEZ_MIN_CTAS
 #define DEODR_TILEZ_MIN_CTAS 6  // H100 (400 W), 1M-triangle scene: k_tile_z 145 us at 4, 129 us at 5, 126 us at 6
+#endif
+// -DDEODR_TILEZ_PHASE_CLOCKS (measurement builds only, scripts/tilez_phases.py): lane 0 of every warp of a busy tile
+// adds the clock64() cycles it spent in each phase of k_tile_z to g_tilez_clocks, and thread 0 counts the tile's
+// records in g_tilez_hist.  Read back (and cleared) with deodr_b200_tilez_phase_clocks.
+enum { TZ_COPY_WAIT, TZ_SCATTER, TZ_BARRIER, TZ_PIX_TEST, TZ_LARGE, TZ_EPILOGUE, TZ_TMA_STORE, TZ_PHASES };
+#ifdef DEODR_TILEZ_PHASE_CLOCKS
+constexpr int TZ_HIST = 1025;  // records per busy tile: 0..1023, then >= 1024
+__device__ unsigned long long g_tilez_clocks[TZ_PHASES + 1];  // + warps counted
+__device__ unsigned int g_tilez_hist[TZ_HIST];
+#define TZ_LAP(k)                                  \
+    do {                                           \
+        const long long tz_now_ = clock64();       \
+        tz_acc[k] += (unsigned long long)(tz_now_ - tz_prev); \
+        tz_prev = tz_now_;                         \
+    } while (0)
+#else
+#define TZ_LAP(k) ((void)0)
 #endif
 // PERSP: perspective_correct as a compile-time constant (the 1/z division and its registers leave the common instance).
 // FUSE: the colour of every pixel is computed in this kernel's epilogue (the owner stays in registers: no owner map
@@ -300,7 +320,13 @@ __global__ void __launch_bounds__(NT, DEODR_TILEZ_MIN_CTAS) k_tile_z(SceneView s
     const int n_small = min(c_small, o_end - o_begin);
     const PreRec *list = bins.small_recs + o_begin;
     const int n_chunks = (n_small + PRE_CHUNK - 1) / PRE_CHUNK;
-    sh.tri.pix_cnt[tid] = 0;
+#ifdef DEODR_TILEZ_PHASE_CLOCKS
+    unsigned long long tz_acc[TZ_PHASES] = {};
+    long long tz_prev = clock64();
+    if (tid == 0) atomicAdd(&g_tilez_hist[min(n_small, TZ_HIST - 1)], 1u);
+#endif
+    // (the candidate counters are only used by chunks above WARP_TEST_MAX records, and the first chunk is the largest)
+    if (n_small > WARP_TEST_MAX) sh.tri.pix_cnt[tid] = 0;
     if (tid == 0) {
         mbar_init(&bar[0], 1);
         mbar_init(&bar[1], 1);
@@ -325,17 +351,29 @@ __global__ void __launch_bounds__(NT, DEODR_TILEZ_MIN_CTAS) k_tile_z(SceneView s
         const int m = min(PRE_CHUNK, n_small - chunk * PRE_CHUNK);
         if (b == 0) { mbar_wait(&bar[0], parity0); parity0 ^= 1u; }
         else        { mbar_wait(&bar[1], parity1); parity1 ^= 1u; }
-        phase_pre_scatter<DevEnv>(tid, m, pre[b], &sh);
-        __syncthreads();
-        phase_pix_test<1>(s, tid, m, tile, pre[b], &sh, &p);  // (pixels outside the image have no candidates)
+        TZ_LAP(TZ_COPY_WAIT);
+        // (pixels outside the image have no candidates)
+        if (m <= WARP_TEST_MAX) {  // CTA-uniform: each warp tests its own two rows, no barrier
+            phase_warp_test<1>(s, tid, m, tile, pre[b], &p);
+            TZ_LAP(TZ_PIX_TEST);
+        } else {
+            phase_pre_scatter<DevEnv>(tid, m, pre[b], &sh);
+            TZ_LAP(TZ_SCATTER);
+            __syncthreads();
+            TZ_LAP(TZ_BARRIER);
+            phase_pix_test<1>(s, tid, m, tile, pre[b], &sh, &p);
+            TZ_LAP(TZ_PIX_TEST);
+        }
         if (chunk + 1 < n_chunks) {
             // every pixel is done with buffer b and with its candidate list: the next chunk may be scattered, and the
             // chunk after it may land in buffer b while that one is tested
             __syncthreads();
+            TZ_LAP(TZ_BARRIER);
             if (tid == 0 && chunk + 2 < n_chunks) issue(chunk + 2);
         }
         // (after the last chunk: the large-triangle phases use other fields of sh, the epilogue ends with a barrier)
     }
+    TZ_LAP(TZ_COPY_WAIT);
     // large triangles: by index, stencil set-up and row spans computed here, one thread per triangle
     const int n_large = min(c_large, bins.large.offset[tile_id + 1] - bins.large.offset[tile_id]);
     if (n_large > 0) {
@@ -350,6 +388,7 @@ __global__ void __launch_bounds__(NT, DEODR_TILEZ_MIN_CTAS) k_tile_z(SceneView s
             if (inside) phase_tri_test<1>(s, tid, m, tile, &sh, &p);
         }
     }
+    TZ_LAP(TZ_LARGE);
     if (inside) {
         const size_t idx = (size_t)y * s.width + x;
         z_buffer[idx] = p.z;
@@ -387,6 +426,7 @@ __global__ void __launch_bounds__(NT, DEODR_TILEZ_MIN_CTAS) k_tile_z(SceneView s
     const bool other = inside && p.bown >= 0 && !(p.bown & SMALL_FLAG);
     if (FUSE && MAXC <= 4 && tma_store) fence_proxy_async();  // this thread's staged colours -> visible to the TMA engine
     const bool listed = __syncthreads_or(other);
+    TZ_LAP(TZ_EPILOGUE);
     if (tid == 0) {
         if (listed) large_tiles[atomicAdd(scal + SC_LARGE_TILES, 1)] = tile_id;
         if (FUSE && MAXC <= 4 && tma_store) {
@@ -395,6 +435,13 @@ __global__ void __launch_bounds__(NT, DEODR_TILEZ_MIN_CTAS) k_tile_z(SceneView s
             tma_store_wait_read();  // the staging buffer must outlive the copy engine's read
         }
     }
+#ifdef DEODR_TILEZ_PHASE_CLOCKS
+    TZ_LAP(TZ_TMA_STORE);
+    if (tid % 32 == 0) {
+        for (int k = 0; k < TZ_PHASES; k++) atomicAdd(&g_tilez_clocks[k], tz_acc[k]);
+        atomicAdd(&g_tilez_clocks[TZ_PHASES], 1ull);
+    }
+#endif
 }
 
 // Forward, kernel 2 of 3 - colour of every pixel from its owner (one thread per pixel, tile-shaped blocks for
@@ -1412,6 +1459,23 @@ extern "C" {
 
 const char *deodr_b200_last_error(void) { return deodr_error_buffer(); }
 const char *deodr_b200_version(void) { return "deodr_b200 0.2 (sm_90a)"; }
+
+#ifdef DEODR_TILEZ_PHASE_CLOCKS
+// Measurement builds only: copies k_tile_z's per-phase cycle sums (TZ_PHASES + 1: the last one counts the warps) and
+// its records-per-tile histogram (TZ_HIST) out of the device, then clears them.  Synchronises the device.
+int deodr_b200_tilez_phase_clocks(unsigned long long *clocks, unsigned int *hist) {
+    if (cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpyFromSymbol(clocks, g_tilez_clocks, sizeof(g_tilez_clocks)) != cudaSuccess ||
+        cudaMemcpyFromSymbol(hist, g_tilez_hist, sizeof(g_tilez_hist)) != cudaSuccess)
+        return DEODR_B200_ECUDA;
+    static const unsigned long long zc[TZ_PHASES + 1] = {};
+    static const unsigned int zh[TZ_HIST] = {};
+    if (cudaMemcpyToSymbol(g_tilez_clocks, zc, sizeof(zc)) != cudaSuccess ||
+        cudaMemcpyToSymbol(g_tilez_hist, zh, sizeof(zh)) != cudaSuccess)
+        return DEODR_B200_ECUDA;
+    return DEODR_B200_OK;
+}
+#endif
 
 const char *deodr_b200_phase_name(int phase) {
     static const char *names[] = {"plan",     "edge_bin",      "bin",          "edge_tile_sort", "tile_z",       "shade",

@@ -18,6 +18,13 @@ constexpr int PRE_CHUNK = 128;    // pre-masked records per TMA bulk copy (doubl
 #endif
 constexpr int LARGE_CHUNK = DEODR_LARGE_CHUNK;  // large triangles staged per pass (stencil records kept in shared memory)
 constexpr int PIX_SLOTS = 8;      // candidate small triangles kept per pixel and chunk before the pixel falls back to a scan
+#ifndef DEODR_WARP_TEST_MAX
+#define DEODR_WARP_TEST_MAX 64
+#endif
+// Chunks of at most this many records are z-tested warp by warp (phase_warp_test: no candidate lists, no CTA barrier);
+// larger ones go through the candidate scatter (phase_pre_scatter + phase_pix_test).  H100 (400 W), 1M-triangle scene:
+// k_tile_z 125 us with every chunk scattered, 108 at 64, 110 at 128 (DESIGN.md sections 4 and 9).
+constexpr int WARP_TEST_MAX = DEODR_WARP_TEST_MAX;
 constexpr int EDGE_CHUNK = 64;    // edge records staged in shared memory per pass
 #ifndef DEODR_EDGE_ROWS
 #define DEODR_EDGE_ROWS 16
@@ -538,6 +545,48 @@ DEODR_HD void phase_pix_test(const SceneView &s, int tid, int n, Tile tile, cons
         const int lane = tid % 32, pair = tid / 32;
         for (int t = 0; t < n; t++)
             if ((pre[t].mask[pair] >> lane) & 1u) z_candidate<MAXC>(pre[t].zp, pre[t].id, xd, yd, x, y, persp, p);
+    }
+}
+
+// Candidates of pixel `tid` among records [g, g + 32) of a chunk of n: bit j <=> record g + j covers the pixel.  Mask
+// word p of a record covers tile rows 2p and 2p + 1, i.e. exactly the 32 pixels of warp p (bit = lane), so a warp finds
+// its pixels' candidates from word p of each record alone.  On the device, lane j reads word p of record g + j: word p
+// of every record sits in banks p and p + 16 (64-byte records), so ANY pattern needs m / 2 wavefronts for m records -
+// the one load reaches that (broadcast reads would take m) - then the warp ballots the non-empty words and hands each to
+// every lane by a shuffle.  The host form reads the same bits directly.
+DEODR_HD uint32_t warp_candidates(int tid, int n, int g, const PreRec *pre) {
+    const int lane = tid % 32, pair = tid / 32;
+#if defined(__CUDA_ARCH__)
+    const uint32_t w = g + lane < n ? pre[g + lane].mask[pair] : 0u;
+    uint32_t busy = __ballot_sync(0xffffffffu, w != 0u);
+    uint32_t cand = 0u;
+    while (busy) {  // warp-uniform: one shuffle per record that touches the warp's two rows
+        const int j = __ffs(busy) - 1;
+        busy &= busy - 1;
+        cand |= ((__shfl_sync(0xffffffffu, w, j) >> lane) & 1u) << j;
+    }
+    return cand;
+#else
+    uint32_t cand = 0u;
+    for (int j = 0; j < 32 && g + j < n; j++) cand |= ((pre[g + j].mask[pair] >> lane) & 1u) << j;
+    return cand;
+#endif
+}
+
+// Phase T2a, warp-local form for chunks of at most WARP_TEST_MAX records: no candidate lists and no CTA barrier - a
+// warp waits only for the chunk's copy, and each pixel z-tests its own candidates (any order: ties are resolved by
+// index, so the result is the one phase_pre_scatter + phase_pix_test give).  Every lane of the warp must call it
+// (shuffles), pixels outside the image included: they have no candidates.
+template <int MAXC>
+DEODR_HD void phase_warp_test(const SceneView &s, int tid, int n, Tile tile, const PreRec *pre, PixelState<MAXC> *p) {
+    const int x = tile.x0 + tid % TS, y = tile.y0 + tid / TS;
+    const double xd = (double)x, yd = (double)y;
+    const bool persp = s.perspective_correct != 0;
+    for (int g = 0; g < n; g += 32) {
+        for (uint32_t cand = warp_candidates(tid, n, g, pre); cand; cand &= cand - 1) {
+            const PreRec &r = pre[g + lowest_bit(cand)];
+            z_candidate<MAXC>(r.zp, r.id, xd, yd, x, y, persp, p);
+        }
     }
 }
 
