@@ -1458,7 +1458,12 @@ static int render_b_views_impl(DeodrWorkspace *ws, int n_views, const DeodrScene
 extern "C" {
 
 const char *deodr_b200_last_error(void) { return deodr_error_buffer(); }
+// names the DEODR_EXACT_SHORT_WRAP=1 build (rmath.h): callers can tell which far-vertex behaviour they get
+#if DEODR_EXACT_SHORT_WRAP
+const char *deodr_b200_version(void) { return "deodr_b200 0.2 (sm_90a, exact short wrap)"; }
+#else
 const char *deodr_b200_version(void) { return "deodr_b200 0.2 (sm_90a)"; }
+#endif
 
 #ifdef DEODR_TILEZ_PHASE_CLOCKS
 // Measurement builds only: copies k_tile_z's per-phase cycle sums (TZ_PHASES + 1: the last one counts the warps) and

@@ -57,21 +57,23 @@ DEODR_HD void inv3x3(const double *S, double *T) {
 
 // Vertices beyond the `short` range (more than 32767 pixels from the origin).  The reference's casts wrap there
 // (x86: cvttsd2si to int32, low 16 bits kept; 0x80000000 for anything outside int32), and a triangle with one far
-// vertex is still drawn in part.  DEODR_EXACT_SHORT_WRAP=1 reproduces that bit for bit (validated on the CPU emulation
-// against the compiled reference up to 1e15 px: tests/test_emul.py, scripts/probe_far_vertices.py); the default (0) is
-// the build every GPU measurement and parity run of round 2 was made with: identical below the limit, such triangles
-// are culled beyond it (INTEGRATION.md section 5).  Flip it after one `pytest -m gpu` run of that build.
+// vertex is still drawn in part.  DEODR_EXACT_SHORT_WRAP=1 reproduces that bit for bit (on the CPU emulation against
+// the compiled reference up to 1e15 px, tests/test_emul.py; on an H100, tests/test_gpu_edge_cases.py, where that build
+// passes every `pytest -m gpu` test the default one passes); the default (0) is identical below the limit and culls such
+// triangles beyond it (INTEGRATION.md section 5).  Both builds convert alike (to_short / to_int_trunc below), so they
+// differ only in tri_bounds / tri_geom: same ptxas figures except k_small_tri_bwd<3, false> (63 registers in the exact
+// build, 64 in the default), and the same bench.py c5 speed within run-to-run noise (DESIGN.md section 9).  Making it the default
+// changes which pixels far triangles cover: a behaviour change of its own, not made here.
 #ifndef DEODR_EXACT_SHORT_WRAP
 #define DEODR_EXACT_SHORT_WRAP 0
 #endif
 
 // (short) conversion of the reference: double -> int32 (truncation) -> low 16 bits, sign-extended.
+// In every build: the host and the device must agree on a vertex at 2^31 px or +inf (tests/test_gpu_edge_cases.py).
 DEODR_HD int to_short(double v) {
-#if DEODR_EXACT_SHORT_WRAP
     // cvttsd2si gives 0x80000000 (low 16 bits: 0) outside int32; cvt.rzi.s32.f64 saturates: only the positive side
     // differs in the low 16 bits (0x7fffffff -> -1).  (NaN: 0x80000000 there, 0 here: both 0.)
     if (v >= 2147483648.0) return 0;
-#endif
 #if defined(__CUDA_ARCH__)
     int i = __double2int_rz(v);
 #else
@@ -81,10 +83,10 @@ DEODR_HD int to_short(double v) {
 }
 
 // (int) conversion as the reference's compiler performs it (cvttsd2si): INT_MIN for NaN and anything outside int32.
+// (cvt.rzi.s32.f64 gives INT_MAX from 2^31 up: the band of an edge with such an end point would reach the last
+// image row on the device, where the reference's is empty.)
 DEODR_HD int to_int_trunc(double v) {
-#if DEODR_EXACT_SHORT_WRAP
     if (!(v > -2147483649.0 && v < 2147483648.0)) return (int)0x80000000;
-#endif
 #if defined(__CUDA_ARCH__)
     return __double2int_rz(v);
 #else
