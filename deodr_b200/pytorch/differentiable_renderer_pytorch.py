@@ -17,11 +17,23 @@ and the fitting step of the reference's ``Scene2D.render_compare_and_backward`` 
 
 * ``CudaRenderCompare2D`` - ``(ij, colors, obs, mask, scene, sigma, antialiase_error) -> loss``, the render compared
   with an observed image on the device.
+
+and their textured counterparts, differentiable in all five per-scene inputs of the rasteriser's adjoint (the
+reference's 2D Function returns ``(ij_b, colors_b)`` only; its ``Scene2D`` computes ``uv_b``, ``shade_b`` and
+``texture_b`` but no Function exposes them):
+
+* ``CudaDifferentiableRender2DTextured`` - ``(ij, colors, uv, shade, texture, scene, sigma) -> image``;
+* ``CudaRenderCompare2DTextured`` - ``(ij, colors, uv, shade, texture, obs, mask, scene, sigma, antialiase_error)
+  -> loss``.
+
+Their texture gradient is the summed adjoint of the bilinear sample (the reference's overwrites, INTEGRATION.md
+section 5).  Backward returns only the gradients autograd asks for, and leaves the texture's adjoint slot NULL (not
+computed) when its gradient is not asked for.
 """
 
 from __future__ import annotations
 
-from typing import Any
+from typing import Any, Dict, Optional
 
 import numpy as np
 import torch
@@ -177,3 +189,117 @@ class CudaRenderCompare2DFunc(torch.autograd.Function):
 
 
 CudaRenderCompare2D = CudaRenderCompare2DFunc.apply
+
+
+TEXTURED_INPUTS = ("ij", "colors", "uv", "shade", "texture")
+
+
+def check_scene_inputs(scene: DeviceScene, **inputs: torch.Tensor) -> None:
+    """``ValueError`` unless every tensor is a CUDA tensor of the shape the ``DeviceScene`` holds under its name."""
+    for name, t in inputs.items():
+        want = tuple(scene.t[name].shape)
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise ValueError(f"{name} must be a CUDA tensor of shape {want}")
+        if tuple(t.shape) != want:
+            raise ValueError(f"{name} has shape {tuple(t.shape)}; the scene expects {want}")
+
+
+def requested_grads(scene: DeviceScene, names, needs) -> Dict[str, torch.Tensor]:
+    """Zeroed fp32 gradient slots ``{name + "_b": ...}`` for the adjoint of a textured scene.  The library needs the
+    ij, colour, uv and shade slots; the texture slot, the only one it may leave NULL (and the largest), is allocated
+    only when ``needs`` asks for the texture gradient (``names`` and ``needs`` as the Function's inputs)."""
+    want_texture = dict(zip(names, needs)).get("texture", False)
+    return {n + "_b": torch.zeros(scene.t[n].shape, dtype=torch.float32, device=scene.device)
+            for n in TEXTURED_INPUTS if n != "texture" or want_texture}
+
+
+def gradients_of(grads: Dict[str, torch.Tensor], names, dtypes, needs,
+                 scale: Optional[torch.Tensor] = None) -> tuple:
+    """The gradients of ``names`` in their inputs' dtypes (times ``scale``), None where ``needs`` asks for none."""
+    out = []
+    for n, dtype, need in zip(names, dtypes, needs):
+        g = grads[n + "_b"] if need else None
+        if g is not None and scale is not None:
+            g = g * scale
+        out.append(g.to(dtype) if g is not None else None)
+    return tuple(out)
+
+
+class CudaDifferentiableRenderer2DTexturedFunc(torch.autograd.Function):
+    """``image = f(ij [V,2], colors [V,C], uv [Nuv,2], shade [V], texture [Ht,Wt,C], DeviceScene, sigma)`` on the
+    device, CUDA tensors shaped like the scene's.  Backward returns the gradient of each of the five inputs that needs
+    one, in its own dtype (None for the others), then ``None, None``.  Same snapshot / re-render logic as
+    ``CudaDifferentiableRenderer2DFunc``, over all five inputs."""
+
+    @staticmethod
+    def forward(ctx: Any, ij: torch.Tensor, colors: torch.Tensor, uv: torch.Tensor, shade: torch.Tensor,  # type: ignore
+                texture: torch.Tensor, scene: DeviceScene, sigma: float = 1.0):
+        inputs = dict(zip(TEXTURED_INPUTS, (ij, colors, uv, shade, texture)))
+        check_scene_inputs(scene, **inputs)
+        scene.update(**{k: t.detach() for k, t in inputs.items()})
+        fwd = default_renderer(scene.device.index).render(scene, sigma)
+        ctx.scene, ctx.sigma, ctx.fwd = scene, float(sigma), fwd
+        ctx.in_dtypes = tuple(t.dtype for t in inputs.values())
+        ctx.save_for_backward(*(t.detach().clone() for t in inputs.values()))
+        # the caller gets its own tensor: the framebuffers of ctx.fwd may be re-rendered into by backward
+        return fwd["image"].clone()
+
+    @staticmethod
+    def backward(ctx: Any, image_b: torch.Tensor):  # type: ignore
+        needs = ctx.needs_input_grad[:5]
+        if not any(needs):
+            return (None,) * 7
+        renderer = default_renderer(ctx.scene.device.index)
+        # the shared scene may hold another node's inputs by now
+        ctx.scene.update(**dict(zip(TEXTURED_INPUTS, ctx.saved_tensors)))
+        if ctx.fwd["generation"] != renderer.generation(ctx.fwd["slot"]):
+            ctx.fwd = renderer.render(ctx.scene, ctx.sigma, out=ctx.fwd)
+        grads = requested_grads(ctx.scene, TEXTURED_INPUTS, needs)
+        renderer.render_b(ctx.scene, ctx.sigma, ctx.fwd, image_b.contiguous(), grads=grads)
+        return gradients_of(grads, TEXTURED_INPUTS, ctx.in_dtypes, needs) + (None, None)
+
+
+CudaDifferentiableRender2DTextured = CudaDifferentiableRenderer2DTexturedFunc.apply
+
+
+class CudaRenderCompare2DTexturedFunc(torch.autograd.Function):
+    """``loss = f(ij, colors, uv, shade, texture, obs [H,W,C], mask [H,W] | None, DeviceScene, sigma,
+    antialiase_error)``: ``CudaRenderCompare2DFunc`` (same loss, both modes, the gradients scaled by ``grad_loss`` on
+    the device) differentiable in the five inputs of ``CudaDifferentiableRenderer2DTexturedFunc``."""
+
+    @staticmethod
+    def forward(ctx: Any, ij: torch.Tensor, colors: torch.Tensor, uv: torch.Tensor, shade: torch.Tensor,  # type: ignore
+                texture: torch.Tensor, obs: torch.Tensor, mask: Any, scene: DeviceScene, sigma: float = 1.0,
+                antialiase_error: bool = False):
+        inputs = dict(zip(TEXTURED_INPUTS, (ij, colors, uv, shade, texture)))
+        check_scene_inputs(scene, **inputs)
+        scene.update(**{k: t.detach() for k, t in inputs.items()})
+        res = default_renderer(scene.device.index).render_compare(scene, sigma, obs, mask,
+                                                                  antialiase_error=antialiase_error)
+        ctx.scene, ctx.sigma, ctx.res, ctx.err_mode = scene, float(sigma), res, bool(antialiase_error)
+        ctx.in_dtypes = tuple(t.dtype for t in inputs.values())
+        ctx.save_for_backward(*(t.detach().clone() for t in inputs.values()), obs, mask)
+        # the caller gets its own scalar: ctx.res may be re-rendered into by backward
+        return res["loss"].clone()
+
+    @staticmethod
+    def backward(ctx: Any, grad_loss: torch.Tensor):  # type: ignore
+        needs = ctx.needs_input_grad[:5]
+        if not any(needs):
+            return (None,) * 10
+        renderer = default_renderer(ctx.scene.device.index)
+        *inputs, obs, mask = ctx.saved_tensors
+        ctx.scene.update(**dict(zip(TEXTURED_INPUTS, inputs)))  # the shared scene may hold another node's inputs
+        if ctx.res["generation"] != renderer.generation(ctx.res["slot"]):
+            ctx.res = renderer.render_compare(ctx.scene, ctx.sigma, obs, mask, antialiase_error=ctx.err_mode,
+                                              out=ctx.res)
+        grads = requested_grads(ctx.scene, TEXTURED_INPUTS, needs)
+        if ctx.err_mode:
+            renderer.render_b(ctx.scene, ctx.sigma, ctx.res, grads=grads,
+                              err_buffer_b=renderer.compare_adjoint_input(ctx.res))
+        else:
+            renderer.render_b(ctx.scene, ctx.sigma, ctx.res, ctx.res["image_b"], grads=grads)
+        return gradients_of(grads, TEXTURED_INPUTS, ctx.in_dtypes, needs, grad_loss.to(torch.float32)) + (None,) * 5
+
+
+CudaRenderCompare2DTextured = CudaRenderCompare2DTexturedFunc.apply

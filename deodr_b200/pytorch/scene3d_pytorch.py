@@ -12,13 +12,15 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
                            -> colours [V,C]
     RenderMesh2DFunc       (ij, colors, depths, edgeflags, DeviceScene, sigma) -> image [H,W,C] fp32
                            gradients to ij and colors (depths get none, as in the reference)
-    PoseFunc               (vertices, quaternion [4], translation [3]) -> qrot(q / |q|, v - mean v) + t
+    RenderMesh2DTexturedFunc  (ij, uv, shade, texture, depths, edgeflags, DeviceScene, sigma) -> image [H,W,C] fp32
+                           gradients to ij, uv, shade and texture (a textured mesh: Scene3D.render's uv branch)
+    PoseFunc              (vertices, quaternion [4], translation [3]) -> qrot(q / |q|, v - mean v) + t
     RigidEnergyFunc        (vertices, DeviceLaplacianRigidEnergy) -> energy 0-d
 
-All maths is fp64 but the rasteriser's (fp32 image and image gradients).  ``RenderMesh2DFunc`` follows the snapshot /
-replay rule of the 2D Functions (differentiable_renderer_pytorch.py): the renderer keeps one forward state per slot,
-so if another forward has used the slot before ``backward`` runs, the forward is replayed from the node's own copy of
-its inputs (depths and edge flags included).
+All maths is fp64 but the rasteriser's (fp32 image and image gradients).  ``RenderMesh2DFunc`` and
+``RenderMesh2DTexturedFunc`` follow the snapshot / replay rule of the 2D Functions (differentiable_renderer_pytorch.py):
+the renderer keeps one forward state per slot, so if another forward has used the slot before ``backward`` runs, the
+forward is replayed from the node's own copy of its inputs (depths and edge flags included).
 """
 
 from __future__ import annotations
@@ -32,6 +34,7 @@ from ..mesh_fitter import DeviceLaplacianRigidEnergy, new_scratch, pose, pose_ba
 from ..mesh_ops import (CameraParams, MeshTopology, lit_vertex_colors, lit_vertex_colors_backward, project_points,
                         project_points_backward_f64)
 from ..renderer import DeviceScene, default_renderer
+from .differentiable_renderer_pytorch import check_scene_inputs, gradients_of, requested_grads
 
 _scratch: Dict[torch.device, torch.Tensor] = {}
 
@@ -152,6 +155,45 @@ class RenderMesh2DFunc(torch.autograd.Function):
         return grads["ij_b"].to(ctx.in_dtypes[0]), grads["colors_b"].to(ctx.in_dtypes[1]), None, None, None, None
 
 
+class RenderMesh2DTexturedFunc(torch.autograd.Function):
+    """The rasteriser under a textured 3D render: (ij [V,2], uv [Nuv,2], shade [V], texture [Ht,Wt,C], depths [V],
+    edgeflags [T,3], DeviceScene, sigma) -> image [H,W,C] fp32, on a scene whose triangles are all textured and shaded
+    and whose colours are zero.  Backward returns the gradients of ij, uv, shade and texture that autograd asks for
+    (the texture's adjoint slot stays NULL when its gradient is not asked for), none for the depths and edge flags.  Same snapshot / replay rule as
+    ``RenderMesh2DFunc``, over all six inputs."""
+
+    NAMES = ("ij", "uv", "shade", "texture")
+
+    @staticmethod
+    def forward(ctx: Any, ij: torch.Tensor, uv: torch.Tensor, shade: torch.Tensor, texture: torch.Tensor,  # type: ignore
+                depths: torch.Tensor, edgeflags: torch.Tensor, scene: DeviceScene, sigma: float = 1.0):
+        check_scene_inputs(scene, uv=uv, texture=texture)
+        inputs = {"ij": ij.detach(), "uv": uv.detach(), "shade": shade.detach(), "texture": texture.detach(),
+                  "depths": depths.detach(), "edgeflags": edgeflags}
+        scene.update(**inputs)
+        fwd = default_renderer(scene.device.index).render(scene, sigma)
+        ctx.scene, ctx.sigma, ctx.fwd = scene, float(sigma), fwd
+        ctx.in_dtypes = (ij.dtype, uv.dtype, shade.dtype, texture.dtype)
+        ctx.save_for_backward(*(t.clone() for t in inputs.values()))
+        # the caller gets its own tensor: the framebuffers of ctx.fwd may be re-rendered into by backward
+        return fwd["image"].clone()
+
+    @staticmethod
+    def backward(ctx: Any, image_b: torch.Tensor):  # type: ignore
+        names = RenderMesh2DTexturedFunc.NAMES
+        needs = ctx.needs_input_grad[:4]
+        if not any(needs):
+            return (None,) * 8
+        renderer = default_renderer(ctx.scene.device.index)
+        # the shared scene may hold another node's inputs by now
+        ctx.scene.update(**dict(zip(names + ("depths", "edgeflags"), ctx.saved_tensors)))
+        if ctx.fwd["generation"] != renderer.generation(ctx.fwd["slot"]):
+            ctx.fwd = renderer.render(ctx.scene, ctx.sigma, out=ctx.fwd)
+        grads = requested_grads(ctx.scene, names, needs)
+        renderer.render_b(ctx.scene, ctx.sigma, ctx.fwd, image_b.contiguous(), grads=grads)
+        return gradients_of(grads, names, ctx.in_dtypes, needs) + (None,) * 4
+
+
 class PoseFunc(torch.autograd.Function):
     """(vertices [V,3], quaternion [4], translation [3]) -> qrot(q / |q|, v - mean v) + t, fp64 (deodr_b200_pose /
     _pose_b; quaternion stored x, y, z, w).  The input is not modified: the kernel centres a copy."""
@@ -198,8 +240,17 @@ project_points_autograd = ProjectPointsFunc.apply
 vertex_normals_autograd = VertexNormalsFunc.apply
 lit_vertex_colors_autograd = LitVertexColorsFunc.apply
 render_mesh_2d = RenderMesh2DFunc.apply
+render_mesh_2d_textured = RenderMesh2DTexturedFunc.apply
 pose_autograd = PoseFunc.apply
 rigid_energy_autograd = RigidEnergyFunc.apply
+
+
+def vertex_luminosity_autograd(normals: torch.Tensor, light_directional: Optional[torch.Tensor],
+                               light_ambient: torch.Tensor) -> torch.Tensor:
+    """``Scene3D.compute_vertices_luminosity``: [V] fp64 = relu(-<n, l>) + ambient, :class:`LitVertexColorsFunc` on a
+    column of ones (the same arithmetic as ``mesh_ops.vertex_luminosity``, rounded to fp32 only by the rasteriser)."""
+    ones = torch.ones((normals.shape[0], 1), dtype=torch.float64, device=normals.device)
+    return lit_vertex_colors_autograd(normals, ones, light_directional, light_ambient)[:, 0]
 
 
 # ---- the reference's classes ------------------------------------------------------------------------------------------
@@ -228,9 +279,15 @@ class CameraPytorch(CameraParams):
 class ColoredTriMeshPytorch:
     """``deodr.pytorch.ColoredTriMeshPytorch(faces, vertices, clockwise=False, colors=None)`` on the device: the
     vertices [V,3] and vertex colours [V,C] are CUDA tensors (either may require grad), the adjacency a
-    :class:`MeshTopology` built once.  Untextured meshes only."""
+    :class:`MeshTopology` built once.
 
-    def __init__(self, faces, vertices, clockwise: bool = False, colors=None, device=None):
+    ``faces_uv`` [T,3], ``uv`` [Nuv,2] and ``texture`` [Ht,Wt,C], given together, make the mesh textured, in the
+    conventions of the reference's ``ColoredTriMesh`` (uv in texel units).  ``uv`` and ``texture`` are tensors (fp32 or
+    fp64, either may require grad) or arrays, uploaded once; the attributes ``uv`` and ``texture`` may be reassigned
+    between renders."""
+
+    def __init__(self, faces, vertices, clockwise: bool = False, colors=None, device=None, faces_uv=None, uv=None,
+                 texture=None):
         self.device = _device(device if device is not None else
                               (vertices.device if isinstance(vertices, torch.Tensor) else None))
         self.faces = np.ascontiguousarray(np.asarray(faces), dtype=np.int64)
@@ -242,6 +299,24 @@ class ColoredTriMeshPytorch:
         self.vertices_colors = None
         if colors is not None:
             self.set_vertices_colors(colors)
+        self.faces_uv = self.uv = self.texture = None
+        if faces_uv is not None or uv is not None or texture is not None:
+            if faces_uv is None or uv is None or texture is None:
+                raise ValueError("a textured mesh needs faces_uv, uv and texture together")
+            self.uv, self.texture = self._tensor(uv), self._tensor(texture)
+            self.faces_uv = np.ascontiguousarray(np.asarray(faces_uv), dtype=np.int64)
+            if self.texture.dim() != 3:
+                raise ValueError(f"texture must be [Ht,Wt,C]; got shape {tuple(self.texture.shape)}")
+            if self.uv.dim() != 2 or self.uv.shape[1] != 2 or self.faces_uv.shape != self.faces.shape:
+                raise ValueError(f"uv must be [Nuv,2] and faces_uv [T,3] like faces = {self.faces.shape}; got "
+                                 f"{tuple(self.uv.shape)} and {self.faces_uv.shape}")
+            # the rasteriser reads uv through faces_uv unchecked
+            if self.faces_uv.size and (self.faces_uv.min() < 0 or self.faces_uv.max() >= self.uv.shape[0]):
+                raise ValueError(f"faces_uv indices must lie in [0, {self.uv.shape[0]})")
+
+    @property
+    def textured(self) -> bool:
+        return self.faces_uv is not None
 
     def _tensor(self, a) -> torch.Tensor:
         if isinstance(a, torch.Tensor):
@@ -263,7 +338,8 @@ class ColoredTriMeshPytorch:
 class Scene3DPytorch:
     """``deodr.pytorch.Scene3DPytorch`` on the device: ``set_mesh``, ``set_light(light_directional, light_ambient)``,
     ``set_background_color``, ``render(camera)`` -> image [H,W,C] and ``render_depth(camera, depth_scale)`` -> [H,W,1],
-    fp32 CUDA tensors differentiable in the mesh's vertices and colours and in the light (untextured meshes).
+    fp32 CUDA tensors differentiable in the mesh's vertices and colours (or uv and texture, for a textured mesh) and in
+    the light.
 
     A render is the chain of Functions of this module; ``sigma`` is the antialiasing width of the reference's Scene3D
     (1 by default; at 0 no silhouette edge is drawn).  The backgrounds are set on the device by
@@ -298,7 +374,10 @@ class Scene3DPytorch:
             if scene.nb_colors == self.background_color.shape[0]:
                 scene.t["background_color"].copy_(torch.from_numpy(self.background_color))
 
-    def _scene(self, camera: CameraPytorch, nb_colors: int) -> DeviceScene:
+    def _scene(self, camera: CameraPytorch, nb_colors: int, uv: Optional[torch.Tensor] = None,
+               texture: Optional[torch.Tensor] = None) -> DeviceScene:
+        """The cached 2D scene of the mesh for ``camera``: untextured, or with ``uv`` / ``texture`` given, textured
+        (all triangles textured and shaded, colours zero; the mesh's faces_uv uploaded with it)."""
         from ..scenes import SceneArrays
 
         if self.background_color is None:
@@ -306,18 +385,22 @@ class Scene3DPytorch:
         if self.background_color.shape[0] != nb_colors:
             raise ValueError(f"the background colour has {self.background_color.shape[0]} entries and the render "
                              f"{nb_colors} channels")
-        key = (camera.height, camera.width, nb_colors)
+        textured = texture is not None
+        key = (camera.height, camera.width, nb_colors) + ((tuple(texture.shape), uv.shape[0]) if textured else ())
         if key not in self._scenes:
             m = self.mesh
             T, V = m.nb_faces, m.nb_vertices
             faces = np.ascontiguousarray(m.faces, dtype=np.uint32)
+            flags = np.full(T, textured)
             self._scenes[key] = DeviceScene(SceneArrays(
-                faces=faces, faces_uv=faces, ij=np.zeros((V, 2)), depths=np.ones(V), textured=np.zeros(T, bool),
-                uv=np.zeros((V, 2)), shade=np.zeros(V), colors=np.zeros((V, nb_colors)), shaded=np.zeros(T, bool),
-                edgeflags=np.zeros((T, 3), bool), height=camera.height, width=camera.width, nb_colors=nb_colors,
-                texture=np.zeros((2, 2, nb_colors)), background_image=None, background_color=self.background_color,
-                clockwise=m.clockwise, backface_culling=self.backface_culling, strict_edge=True,
-                perspective_correct=False, integer_pixel_centers=True), m.device)
+                faces=faces, faces_uv=np.ascontiguousarray(m.faces_uv, dtype=np.uint32) if textured else faces,
+                ij=np.zeros((V, 2)), depths=np.ones(V), textured=flags,
+                uv=np.zeros((uv.shape[0] if textured else V, 2)), shade=np.zeros(V), colors=np.zeros((V, nb_colors)),
+                shaded=flags, edgeflags=np.zeros((T, 3), bool), height=camera.height, width=camera.width,
+                nb_colors=nb_colors, texture=np.zeros(tuple(texture.shape) if textured else (2, 2, nb_colors)),
+                background_image=None, background_color=self.background_color, clockwise=m.clockwise,
+                backface_culling=self.backface_culling, strict_edge=True, perspective_correct=False,
+                integer_pixel_centers=True), m.device)
         return self._scenes[key]
 
     def _edgeflags(self, ij: torch.Tensor) -> torch.Tensor:
@@ -333,14 +416,39 @@ class Scene3DPytorch:
             (m.nb_vertices, 3), dtype=torch.float64, device=m.device)
         return lit_vertex_colors_autograd(normals, m.vertices_colors, self.light_directional, self.light_ambient)
 
+    def _compute_vertices_luminosity(self) -> torch.Tensor:
+        m = self.mesh
+        if self.light_ambient is None:
+            raise ValueError("set_light first")
+        normals = m.vertex_normals if self.light_directional is not None else torch.zeros(
+            (m.nb_vertices, 3), dtype=torch.float64, device=m.device)
+        return vertex_luminosity_autograd(normals, self.light_directional, self.light_ambient)
+
     def render(self, camera: CameraPytorch) -> torch.Tensor:
-        """The mesh's vertex colours, Gouraud-lit, rendered by ``camera`` -> image [H,W,C] fp32."""
+        """The mesh's vertex colours, Gouraud-lit, rendered by ``camera`` -> image [H,W,C] fp32.  For a textured mesh,
+        ``Scene3D.render``'s uv branch: the texture, sampled at the interpolated uv, times the interpolated vertex
+        luminosity (differentiable in the vertices, uv, texture and light)."""
+        if self.mesh is not None and self.mesh.textured:
+            return self._render_textured(camera)
         if self.mesh is None or self.mesh.vertices_colors is None:
             raise ValueError("render needs a mesh with vertex colours (set_mesh, set_vertices_colors)")
         ij, depths = camera.project_points(self.mesh.vertices)
         colors = self._compute_vertices_colors_with_illumination()
         scene = self._scene(camera, colors.shape[1])
         return render_mesh_2d(ij, colors, depths, self._edgeflags(ij), scene, self.sigma)
+
+    def _render_textured(self, camera: CameraPytorch) -> torch.Tensor:
+        m = self.mesh
+        uv, texture = m._tensor(m.uv), m._tensor(m.texture)
+        if texture.dim() != 3 or uv.dim() != 2 or uv.shape[1] != 2:
+            raise ValueError(f"a textured mesh needs texture [Ht,Wt,C] and uv [Nuv,2]; got {tuple(texture.shape)} and "
+                             f"{tuple(uv.shape)}")
+        if m.faces_uv.size and int(m.faces_uv.max()) >= uv.shape[0]:
+            raise ValueError(f"uv has {uv.shape[0]} rows; faces_uv indexes row {int(m.faces_uv.max())}")
+        ij, depths = camera.project_points(m.vertices)
+        shade = self._compute_vertices_luminosity()
+        scene = self._scene(camera, texture.shape[2], uv=uv, texture=texture)
+        return render_mesh_2d_textured(ij, uv, shade, texture, depths, self._edgeflags(ij), scene, self.sigma)
 
     def render_depth(self, camera: CameraPytorch, depth_scale: float = 1.0) -> torch.Tensor:
         """``Scene3D.render_depth``: a one-channel image [H,W,1] fp32 whose colour is the vertex depth times
