@@ -650,7 +650,7 @@ DEODR_HD void phase_tri_test(const SceneView &s, int tid, int n, Tile tile, cons
 // Phase S: background + owner colour.
 template <int MAXC>
 DEODR_HD void phase_shade(const SceneView &s, int x, int y, PixelState<MAXC> *p, float *w_out = nullptr) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     if (w_out) w_out[0] = w_out[1] = w_out[2] = 0.0f;
     if (p->own < 0) {
         if (s.background_image) {
@@ -1008,7 +1008,7 @@ template <int MAXC, class Env>
 DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, const int *edge_tile_count,
                                      const int *owner, const int *tie_pairs, const float *image_b, float *ij_b,
                                      float *colors_b, float *uv_b, float *shade_b, float *texture_b) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     double V[3][2];
     for (int i = 0; i < 3; i++) {
         const uint32_t v = s.faces[3 * k + i];

@@ -37,6 +37,19 @@ struct SceneView {
 // (DESIGN.md section 4).
 constexpr int COLOR_SLAB = 16;
 
+// Channel count seen by a kernel instance compiled for at most MAXC channels.  The <1> and <3> device instances are only
+// launched for exactly 1 / 3 channels (fix_channel_count, kernels_common.cuh, stores that count into the kernel's copy
+// of the scene), but the compiler does not carry that stored constant into the per-channel loops: they stay loops over
+// arrays in local memory (k_small_tri_bwd<3, false>: a 72-byte frame).  Returned as a compile-time constant there, the
+// loops unroll and the arrays live in registers.  (The CPU emulation also runs the <3> instances for 2 channels.)
+template <int MAXC>
+DEODR_HD int channels(const SceneView &s) {
+#if defined(__CUDA_ARCH__)
+    if (MAXC == 1 || MAXC == 3) return MAXC;
+#endif
+    return s.nb_colors;
+}
+
 DEODR_HD double pixel_offset(const SceneView &s) { return s.integer_pixel_centers ? 0.0 : 0.5; }
 
 // Classification of DR.h:2751-2779: depth-sum key, all-vertices-in-front test, signed area on the UN-offset ij.
@@ -213,7 +226,7 @@ struct PixelEval {
 template <int MAXC>
 DEODR_HD void pixel_colour(const SceneView &s, const TriAttr &t, int x, int y, double Z, PixelEval<MAXC> *e,
                            float *colour) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     double wd[3];
     tri_weights(s, t, x, y, Z, wd);
     for (int i = 0; i < 3; i++) e->w[i] = (float)wd[i];
