@@ -520,7 +520,7 @@ __global__ void __launch_bounds__(EDGE_NT, DEODR_EDGE_MIN_CTAS) k_edge_fwd(Scene
             p.z = z_buffer[idx];
             if (ERR) err = err_buffer[idx];
             else
-                for (int k = 0; k < s.nb_colors; k++) p.col[k] = image[idx * s.nb_colors + k];
+                for (int k = 0; k < channels<MAXC>(s); k++) p.col[k] = image[idx * channels<MAXC>(s) + k];
         }
         const int edge_base = et.seg.offset[tile_id];
         for (int base = 0; base < n_edge; base += EDGE_CHUNK) {
@@ -533,7 +533,7 @@ __global__ void __launch_bounds__(EDGE_NT, DEODR_EDGE_MIN_CTAS) k_edge_fwd(Scene
             for (int item = tid; item < m * TS; item += EDGE_NT)
                 span_cache[(size_t)(edge_base + base) * TS + item] = sh.edge.span[item / TS][item % TS];
             if (inside) {
-                if (ERR) phase_edge_blend_error<MAXC>(s, x, y, r, m, &sh, p.z, obs + idx * s.nb_colors, &err);
+                if (ERR) phase_edge_blend_error<MAXC>(s, x, y, r, m, &sh, p.z, obs + idx * channels<MAXC>(s), &err);
                 else phase_edge_blend<MAXC>(s, x, y, r, m, &sh, &p);
             }
             __syncthreads();
@@ -541,7 +541,7 @@ __global__ void __launch_bounds__(EDGE_NT, DEODR_EDGE_MIN_CTAS) k_edge_fwd(Scene
         if (inside) {
             if (ERR) err_buffer[idx] = err;
             else
-                for (int k = 0; k < s.nb_colors; k++) image[idx * s.nb_colors + k] = p.col[k];
+                for (int k = 0; k < channels<MAXC>(s); k++) image[idx * channels<MAXC>(s) + k] = p.col[k];
         }
     }
 }

@@ -106,15 +106,15 @@ __global__ void __launch_bounds__(EDGE_NT, DEODR_EDGE_MIN_CTAS) k_raster_bwd(Sce
             if (inside) {
                 p.z = t_z[tid];
                 decode_owner(t_own[tid], ties, &p.own, &p.bown);
-                for (int k = 0; k < s.nb_colors; k++) a.g[k] = t_img[tid * s.nb_colors + k];
+                for (int k = 0; k < channels<MAXC>(s); k++) a.g[k] = t_img[tid * channels<MAXC>(s) + k];
             }
         } else if (inside) {
             p.z = z_buffer[idx];
             decode_owner(owner[idx], ties, &p.own, &p.bown);
-            for (int k = 0; k < s.nb_colors; k++) a.g[k] = image_b[idx * s.nb_colors + k];
+            for (int k = 0; k < channels<MAXC>(s); k++) a.g[k] = image_b[idx * channels<MAXC>(s) + k];
         }
         if (ERR && inside) ea.g = (double)err_b[idx];
-        const float *obs_px = ERR ? obs + idx * s.nb_colors : nullptr;
+        const float *obs_px = ERR ? obs + idx * channels<MAXC>(s) : nullptr;
 
         {
             const int edge_base = et.seg.offset[tile_id];
@@ -175,13 +175,13 @@ __global__ void __launch_bounds__(EDGE_NT, DEODR_EDGE_MIN_CTAS) k_raster_bwd(Sce
         if constexpr (BG) {
             const bool shows = inside && p.bown == -1;
             if (bg.background_image_b && shows)
-                for (int k = 0; k < s.nb_colors; k++) atomicAdd(bg.background_image_b + idx * s.nb_colors + k, a.g[k]);
+                for (int k = 0; k < channels<MAXC>(s); k++) atomicAdd(bg.background_image_b + idx * channels<MAXC>(s) + k, a.g[k]);
             if (bg.background_color_b) {
                 __shared__ double bg_partial[EDGE_NT / 32][MAXC];
                 float g[MAXC];
 #pragma unroll
                 for (int k = 0; k < MAXC; k++) g[k] = shows ? a.g[k] : 0.0f;
-                background_color_sum<MAXC, EDGE_NT>(s.nb_colors, g, bg.background_color_b, bg_partial);
+                background_color_sum<MAXC, EDGE_NT>(channels<MAXC>(s), g, bg.background_color_b, bg_partial);
             }
         }
     }
@@ -249,7 +249,7 @@ __global__ void __launch_bounds__(NT, DEODR_INTERIOR_MIN_CTAS) k_interior_bwd(Sc
             decode_owner(owner[idx], ties, &p.own, &p.bown);
             if (p.bown >= 0 && (p.bown & SMALL_FLAG)) p.bown = -1;  // taken by k_small_tri_bwd (triangle-parallel)
             if (p.bown >= 0)
-                for (int k = 0; k < s.nb_colors; k++) g[k] = image_b[idx * s.nb_colors + k];
+                for (int k = 0; k < channels<MAXC>(s); k++) g[k] = image_b[idx * channels<MAXC>(s) + k];
         }
         interior_adjoint_warp<MAXC>(s, x, y, inside && p.bown >= 0, p, g, grads);
     }

@@ -31,7 +31,7 @@ template <int MAXC>
 static __device__ __forceinline__ void interior_adjoint_warp(const SceneView &s, int x, int y, bool has,
                                                              const PixelState<MAXC> &p, const float *g,
                                                              const DeodrGrads &grads) {
-    const int lane = (int)(threadIdx.x & 31), C = s.nb_colors;
+    const int lane = (int)(threadIdx.x & 31), C = channels<MAXC>(s);
     TriAttr t;
     VertexGrads<MAXC> acc;
     zero_vertex_grads<MAXC>(s, &acc);

@@ -758,7 +758,7 @@ DEODR_HD unsigned long long edge_hit_mask(const TileShared *sh, int n, int r, in
 // Phase E3 (forward): overdraw in list order.  image = T*image + (1-T)*A where Z_edge < z_buffer (DR.h:1632-1641).
 template <int MAXC>
 DEODR_HD void phase_edge_blend(const SceneView &s, int x, int y, int r, int n, const TileShared *sh, PixelState<MAXC> *p) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     for (unsigned long long mask = edge_hit_mask(sh, n, r, x); mask; mask &= mask - 1) {
         const EdgeRec &rec = sh->edge.rec[lowest_bit64(mask)];
         double ze = edge_z(rec, x, y, s.perspective_correct != 0);
@@ -785,7 +785,7 @@ struct AdjointState {
 template <int MAXC>
 DEODR_HD void phase_edge_replay(const SceneView &s, int x, int y, int r, int n, const TileShared *sh,
                                 const PixelState<MAXC> &p, AdjointState<MAXC> *a) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     for (unsigned long long mask = edge_hit_mask(sh, n, r, x); mask; mask &= mask - 1) {
         const EdgeRec &rec = sh->edge.rec[lowest_bit64(mask)];
         double ze = edge_z(rec, x, y, false);
@@ -807,7 +807,7 @@ DEODR_HD void phase_edge_replay(const SceneView &s, int x, int y, int r, int n, 
 template <int MAXC, class Env>
 DEODR_HD void phase_edge_adjoint(const SceneView &s, int x, int y, int r, int n, const TileShared *sh,
                                  const PixelState<MAXC> &p, AdjointState<MAXC> *a, double *edge_acc, float *texture_b) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     const int stride = edge_acc_stride(C);
     for (unsigned long long mask = edge_hit_mask(sh, n, r, x); mask;) {  // near to far: highest bit first
         const int e = highest_bit64(mask);
@@ -875,7 +875,7 @@ DEODR_HD void phase_edge_adjoint(const SceneView &s, int x, int y, int r, int n,
 template <int MAXC>
 DEODR_HD double pixel_residual(const SceneView &s, const float *col, const float *obs) {
     double r = 0;
-    for (int c = 0; c < s.nb_colors; c++) {
+    for (int c = 0; c < channels<MAXC>(s); c++) {
         const double d = (double)col[c] - (double)obs[c];
         r += d * d;
     }
@@ -885,7 +885,7 @@ DEODR_HD double pixel_residual(const SceneView &s, const float *col, const float
 template <int MAXC>
 DEODR_HD double edge_residual(const SceneView &s, const EdgeHit<MAXC> &h, const float *obs) {
     double r = 0;
-    for (int c = 0; c < s.nb_colors; c++) {
+    for (int c = 0; c < channels<MAXC>(s); c++) {
         const double d = (double)h.A[c] - (double)obs[c];
         r += d * d;
     }
@@ -925,7 +925,7 @@ DEODR_HD void phase_edge_replay_error(const SceneView &s, int x, int y, int r, i
         if (!a->has) {
             PixelState<MAXC> q = p;
             phase_shade<MAXC>(s, x, y, &q);
-            for (int c = 0; c < s.nb_colors; c++) a->col[c] = q.col[c];
+            for (int c = 0; c < channels<MAXC>(s); c++) a->col[c] = q.col[c];
             a->err = pixel_residual<MAXC>(s, a->col, obs);
             a->has = true;
         }
@@ -943,7 +943,7 @@ template <int MAXC, class Env>
 DEODR_HD void phase_edge_adjoint_error(const SceneView &s, int x, int y, int r, int n, const TileShared *sh,
                                        const PixelState<MAXC> &p, const float *obs, ErrorAdjointState<MAXC> *a,
                                        double *edge_acc, float *texture_b, bool compat) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     const int stride = edge_acc_stride(C);
     for (unsigned long long mask = edge_hit_mask(sh, n, r, x); mask;) {
         const int e = highest_bit64(mask);
@@ -998,7 +998,7 @@ DEODR_HD void phase_edge_adjoint_error(const SceneView &s, int x, int y, int r, 
 // colour adjoint of a pixel from the adjoint of its residual (DR.h:3054-3060)
 template <int MAXC>
 DEODR_HD void residual_adjoint(const SceneView &s, const float *col, const float *obs, double g, float *image_b) {
-    for (int c = 0; c < s.nb_colors; c++) image_b[c] = (float)(-2.0 * ((double)obs[c] - (double)col[c]) * g);
+    for (int c = 0; c < channels<MAXC>(s); c++) image_b[c] = (float)(-2.0 * ((double)obs[c] - (double)col[c]) * g);
 }
 
 // Interior adjoint of one pixel (pixel-parallel kernels): the residual colour adjoint g goes to the vertices of the

@@ -41,7 +41,9 @@ constexpr int COLOR_SLAB = 16;
 // launched for exactly 1 / 3 channels (fix_channel_count, kernels_common.cuh, stores that count into the kernel's copy
 // of the scene), but the compiler does not carry that stored constant into the per-channel loops: they stay loops over
 // arrays in local memory (k_small_tri_bwd<3, false>: a 72-byte frame).  Returned as a compile-time constant there, the
-// loops unroll and the arrays live in registers.  (The CPU emulation also runs the <3> instances for 2 channels.)
+// loops unroll and the arrays live in registers.  The same holds for the edge passes' per-pixel state
+// (k_raster_bwd<3, false, false, false>: a 208-byte frame, 16 with the constant).  (The CPU emulation also runs the
+// <3> instances for 2 channels.)
 template <int MAXC>
 DEODR_HD int channels(const SceneView &s) {
 #if defined(__CUDA_ARCH__)
@@ -265,7 +267,7 @@ DEODR_HD void zero_vertex_grads(const SceneView &s, VertexGrads<MAXC> *a) {
         a->ij[i][0] = a->ij[i][1] = 0.0f;
         a->uv[i][0] = a->uv[i][1] = 0.0f;
         a->shade[i] = 0.0f;
-        for (int c = 0; c < s.nb_colors; c++) a->attr[i][c] = 0.0f;
+        for (int c = 0; c < channels<MAXC>(s); c++) a->attr[i][c] = 0.0f;
     }
 }
 
@@ -275,7 +277,7 @@ DEODR_HD void zero_vertex_grads(const SceneView &s, VertexGrads<MAXC> *a) {
 template <int MAXC, class Env>
 DEODR_HD void pixel_adjoint(const SceneView &s, const TriAttr &t, int x, int y, const float *g, VertexGrads<MAXC> *acc,
                             float *texture_b) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     PixelEval<MAXC> e;
     float colour[MAXC];
     pixel_colour<MAXC>(s, t, x, y, 0.0, &e, colour);
@@ -333,7 +335,7 @@ DEODR_HD void pixel_adjoint(const SceneView &s, const TriAttr &t, int x, int y, 
 template <int MAXC, class Emit>
 DEODR_HD void flush_vertex_grads(const SceneView &s, const TriAttr &t, const VertexGrads<MAXC> &acc, float *ij_b,
                                  float *colors_b, float *uv_b, float *shade_b, const Emit &emit) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     for (int i = 0; i < 3; i++) {
         emit.emit(ij_b + 2 * (size_t)t.vid[i], acc.ij[i][0]);
         emit.emit(ij_b + 2 * (size_t)t.vid[i] + 1, acc.ij[i][1]);
@@ -412,7 +414,7 @@ DEODR_HD double edge_z(const EdgeRec &r, int x, int y, bool persp) {
 
 template <int MAXC>
 DEODR_HD void edge_hit(const SceneView &s, const EdgeRec &r, int x, int y, double Ze, EdgeHit<MAXC> *h) {
-    const int C = s.nb_colors;
+    const int C = channels<MAXC>(s);
     const double *q = r.g.ineq;
     h->b[0] = q[0] * x + q[1] * y + q[2];
     h->b[1] = q[3] * x + q[4] * y + q[5];
