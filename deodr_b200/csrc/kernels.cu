@@ -273,6 +273,33 @@ __device__ unsigned int g_tilez_hist[TZ_HIST];
 #else
 #define TZ_LAP(k) ((void)0)
 #endif
+// -DDEODR_TILEZ_TAIL_CLOCKS (measurement builds only, scripts/step_timeline.py): thread 0 of every CTA of k_tile_z stamps
+// %globaltimer when it starts and when it leaves; g_tilez_tail keeps the earliest start, the latest start and the
+// latest exit.  latest exit - latest start = the kernel's tail after its last CTA was dispatched.  Read back (and
+// reset) with deodr_b200_tilez_tail_clocks.
+#ifdef DEODR_TILEZ_TAIL_CLOCKS
+__device__ unsigned long long g_tilez_tail[3] = {~0ull, 0ull, 0ull};
+static __device__ __forceinline__ unsigned long long global_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+    return t;
+}
+struct TailStamp {
+    __device__ TailStamp() {
+        if (threadIdx.x == 0) {
+            const unsigned long long t = global_ns();
+            atomicMin(&g_tilez_tail[0], t);
+            atomicMax(&g_tilez_tail[1], t);
+        }
+    }
+    __device__ ~TailStamp() {
+        if (threadIdx.x == 0) atomicMax(&g_tilez_tail[2], global_ns());
+    }
+};
+#define TZ_TAIL_STAMP TailStamp tz_tail_stamp_
+#else
+#define TZ_TAIL_STAMP ((void)0)
+#endif
 // PERSP: perspective_correct as a compile-time constant (the 1/z division and its registers leave the common instance).
 // FUSE: the colour of every pixel is computed in this kernel's epilogue (the owner stays in registers: no owner map
 // re-read, no second launch); MAXC / TEX as in k_shade.  The unfused instance <1, PERSP, false, false> + k_shade is
@@ -282,6 +309,7 @@ __global__ void __launch_bounds__(NT, DEODR_TILEZ_MIN_CTAS) k_tile_z(SceneView s
                                                   double *z_buffer, int *owner, int *face_id, int *scal,
                                                   int *large_tiles, float *image, const float *obs, float *err,
                                                   float *bary, const __grid_constant__ TileMap image_map, int tma_store) {
+    TZ_TAIL_STAMP;
     // a list outgrew the plan: the pass is void (the host re-plans and re-runs).  OVF_EDGE_REFS is left out: it is
     // raised by k_bin_edges, which runs beside this kernel, and the early return must be uniform across the CTA
     if (scal[SC_OVERFLOW] & ~OVF_EDGE_REFS) return;
@@ -1487,6 +1515,19 @@ int deodr_b200_tilez_phase_clocks(unsigned long long *clocks, unsigned int *hist
     static const unsigned int zh[TZ_HIST] = {};
     if (cudaMemcpyToSymbol(g_tilez_clocks, zc, sizeof(zc)) != cudaSuccess ||
         cudaMemcpyToSymbol(g_tilez_hist, zh, sizeof(zh)) != cudaSuccess)
+        return DEODR_B200_ECUDA;
+    return DEODR_B200_OK;
+}
+#endif
+
+#ifdef DEODR_TILEZ_TAIL_CLOCKS
+// Measurement builds only: copies k_tile_z's %globaltimer stamps (earliest CTA start, latest CTA start, latest CTA exit,
+// in ns, over every launch since the last call) out of the device, then resets them.  Synchronises the device.
+int deodr_b200_tilez_tail_clocks(unsigned long long *stamps) {
+    static const unsigned long long reset[3] = {~0ull, 0ull, 0ull};
+    if (cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpyFromSymbol(stamps, g_tilez_tail, sizeof(reset)) != cudaSuccess ||
+        cudaMemcpyToSymbol(g_tilez_tail, reset, sizeof(reset)) != cudaSuccess)
         return DEODR_B200_ECUDA;
     return DEODR_B200_OK;
 }

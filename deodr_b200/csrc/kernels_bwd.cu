@@ -350,7 +350,9 @@ template <int MAXC>
 static void launch_bwd(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const SceneView &s, const DeodrViewIO &io,
                        double sigma, int flags, const DeodrGrads &g, const DeodrBackgroundGrads &bg) {
     // Three independent chains (disjoint pixel sets, all accumulate with atomics): edge tiles (longest tail: launched
-    // first so that its CTAs are dispatched first), tiles with large triangles, small triangles.
+    // first, on the lane's high-priority stream, so that its CTAs are dispatched first), tiles with large triangles,
+    // small triangles.  On an equal-priority stream the edge chain's CTAs were dispatched last in a graph replay: on the
+    // 1M-triangle scene k_raster_bwd started 76 us after the adjoint began, and k_finalize_edges ran alone at the end.
     cudaStream_t st = lane.main;
     bool first = true;
     const FwdPlan &plan = v->plan;
@@ -380,7 +382,7 @@ static void launch_bwd(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const SceneV
               encode_tile_map(&maps.owner, io.owner, 4, false, s.height, s.width, TS, TS) &&
               encode_tile_map(&maps.z, io.z_buffer, 8, false, s.height, s.width, TS, TS);
     if (edges) {
-        cudaStream_t se = fork_stream(ws, lane, 1, &first);
+        cudaStream_t se = fork_stream(ws, lane, 0, &first);
         cudaMemsetAsync(v->edge_acc.ptr, 0, (size_t)plan.cap_edges * edge_acc_stride(C) * sizeof(double), se);
         const EdgeTiles et = edge_tiles_of(v);
         const int grid = at_least_one(v->hints_exact && !ws->capturing_internally ? plan.hint_edge_tiles : plan.cap_edge_tiles);
@@ -414,7 +416,7 @@ static void launch_bwd(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const SceneV
         ws->launches++;
     }
     if (bg_on) {  // background pixels of the tiles without silhouette edges (all of them when there are no edges)
-        cudaStream_t sb = fork_stream(ws, lane, 0, &first);
+        cudaStream_t sb = fork_stream(ws, lane, 1, &first);
         PhaseTimer timer(ws, DEODR_B200_PH_BACKGROUND_BWD, sb);
         const size_t pixels = (size_t)s.height * s.width;
         const int grid = at_least_one(std::min(grid_for(pixels, BG_NT), 2048));
@@ -438,9 +440,9 @@ static void launch_bwd(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const SceneV
         }
         ws->launches++;
     }
-    if (edges) join_stream(ws, lane, 1);
+    if (edges) join_stream(ws, lane, 0);
     if (large) join_stream(ws, lane, 2);
-    if (bg_on) join_stream(ws, lane, 0);
+    if (bg_on) join_stream(ws, lane, 1);
 }
 
 

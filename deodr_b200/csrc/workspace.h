@@ -110,7 +110,8 @@ struct ViewSlot {
 };
 
 // One lane = the stream a view's main chain runs on + auxiliary streams for its side chains: aux[0] (high priority)
-// the forward's short silhouette-edge chain, which the main chain waits for; aux[1], aux[2] the adjoint's concurrent kernels.
+// the silhouette-edge chains - the forward's short one, which the main chain waits for, and the adjoint's, whose
+// crowded tiles set the pass's end; aux[1], aux[2] the adjoint's other concurrent kernels (background, large triangles).
 constexpr int LANE_AUX = 3;
 struct Lane {
     cudaStream_t main = nullptr;  // lane 0: the caller's stream (not owned)
