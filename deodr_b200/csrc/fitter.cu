@@ -10,6 +10,7 @@
 //   SH environment     + sh_c(n) beside ambient + diff, per vertex or per pixel                 (+ adjoint)
 //   textured Phong     the same with A read from an albedo raster of its own                    (+ adjoint)
 //   point lights       + P_c(n, x) (and + Q_c per pixel), per vertex or per pixel               (+ adjoint)
+//   shadowed lights    per pixel, light j's terms times a visibility V_j (csrc/scene_ops.cu)    (+ adjoint)
 //   update             heavy-ball steps on the vertices and the few-scalar parameters
 //
 // with qrot(q, v) = v + 2 (w (u x v) + u x (u x v)), u = q_xyz, w = q_w (quaternions stored x, y, z, w).
@@ -900,10 +901,12 @@ __device__ __forceinline__ float &albedo_b_at(float *pb, const DeodrPhongIO &io,
 // separate albedo the default budget spills 8 bytes at S = 1 across the fp64 division calls, so those instances take
 // the registers of one CTA per SM (ptxas -v, DESIGN.md section 12).  With P > 0, point lights [L, 3 + P] add P_c to
 // the luminosity and Q_c to the specular term (P = 1: grey); at P = 3 the default budget spills 12 bytes across the
-// pow calls, so the point-light instances take one CTA's registers too (DESIGN.md section 13)
-template <int S, bool SPLIT, int P = 0>
+// pow calls, so the point-light instances take one CTA's registers too (DESIGN.md section 13).  With VIS (P > 0), light
+// j's diffuse and specular terms are multiplied by its visibility vis [H,W,L] (DESIGN.md section 14)
+template <int S, bool SPLIT, int P = 0, bool VIS = false>
 __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(DeodrPhongIO io, const double *sh,
-                                                                  const float *albedo, const double *lights, int L) {
+                                                                  const float *albedo, const double *lights, int L,
+                                                                  const float *vis = nullptr) {
     const long long p = (long long)blockIdx.x * NT + threadIdx.x;
     if (p >= (long long)io.H * io.W) return;
     const int C = io.C;
@@ -930,6 +933,12 @@ __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(Deod
                 const double *lj = lights + j * (3 + P);
                 PointTerm pt;
                 point_term(lj, x, t.n, true, v, aks, e, pt);
+                if constexpr (VIS) {
+                    // each product rounded on its own, so that V = 1 leaves the terms, and the image, bit for bit
+                    const double vj = vis[p * L + j];
+                    pt.diff = __dmul_rn(pt.diff, vj);
+                    pt.spec = __dmul_rn(pt.spec, vj);
+                }
 #pragma unroll
                 for (int c = 0; c < P; c++) {
                     pd[c] += lj[3 + c] * pt.diff;
@@ -976,11 +985,14 @@ __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(Deod
 // spills a few bytes, so those take the registers of one CTA per SM (ptxas -v, DESIGN.md section 11)
 // With point lights (P > 0) the albedo, normal, position and coverage adjoints, params_b and camera_center_b take their
 // share; lights_b is summed by k_point_lights_pixel_b, a pass of its own (up to 8 (3 + P) sums).
-template <bool CENTER, int S, bool SPLIT, int P = 0>
+// With VIS, light j's terms are scaled by vis [H,W,L] and vis_b[p, j] = alpha_j diff_j + beta_j spec_j is written
+// (0 where a = 0).
+template <bool CENTER, int S, bool SPLIT, int P = 0, bool VIS = false>
 __global__ void __launch_bounds__(NT, S == 2 || S == 4 ? 1 : 0) k_phong_shade_b(DeodrPhongIO io, Scratch *s,
                                                                             const double *sh, const float *albedo,
                                                                             float *albedo_b, const double *lights,
-                                                                            int L) {
+                                                                            int L, const float *vis = nullptr,
+                                                                            float *vis_b = nullptr) {
     constexpr int NC = S > P ? S : P;
     constexpr int K = PHONG_SUMS + (CENTER ? 3 : 0);
     __shared__ double tot[K];
@@ -1062,12 +1074,19 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 ? 1 : 0) k_phong_shade_b(
                     const double *lj = lights + j * (3 + P);
                     PointTerm pt;
                     point_term(lj, x, n, true, v, aks, e, pt);
-                    double alpha = 0, beta = 0, d_b[3] = {0, 0, 0};
+                    double alpha = 0, beta = 0, d_b[3] = {0, 0, 0}, vj = 1.0;
+                    if constexpr (VIS) vj = vis[p * L + j];
+                    const double diff = VIS ? __dmul_rn(pt.diff, vj) : pt.diff;
 #pragma unroll
                     for (int c = 0; c < P; c++) {
                         alpha += gA[c] * lj[3 + c];
                         beta += gs[c] * lj[3 + c];
-                        pd[c] += lj[3 + c] * pt.diff;
+                        pd[c] += lj[3 + c] * diff;
+                    }
+                    if constexpr (VIS) {
+                        vis_b[p * L + j] = (float)(alpha * pt.diff + beta * pt.spec);
+                        alpha = __dmul_rn(alpha, vj);
+                        beta = __dmul_rn(beta, vj);
                     }
                     point_term_b(pt, n, alpha, beta, aks, e, n_b, d_b, v_b, q, e_b);
                     for (int k = 0; k < 3; k++) x_b[k] -= d_b[k];
@@ -1083,6 +1102,8 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 ? 1 : 0) k_phong_shade_b(
                     pX_b[j] = x_b[j] / a;
                 }
                 pa_b -= dot(x_b, x) / a;
+            } else if constexpr (VIS) {
+                for (int j = 0; j < L; j++) vis_b[p * L + j] = 0.0f;
             }
         }
         PhongTerms t;
@@ -1203,10 +1224,11 @@ __global__ void __launch_bounds__(NT) k_phong_sh_b(DeodrPhongIO io, Scratch *s, 
 // lights_b [L, 3 + P] of the Phong forms: CTA (j, y) sums light j over a fixed set of pixels, the position's gradient
 // (the d_j share of k_phong_shade_b) and the intensity's, g_c A_c diff_j + g_c spec_j (P = 1: summed over the
 // channels); grid_sum_rows adds the CTAs in a fixed order.  The CTAs of one set of pixels are adjacent in the grid, so
-// the G-buffer is read from DRAM about once.
-template <int P, bool SPLIT>
+// the G-buffer is read from DRAM about once.  With VIS, light j's terms are scaled by vis [H,W,L].
+template <int P, bool SPLIT, bool VIS = false>
 __global__ void __launch_bounds__(NT) k_point_lights_pixel_b(DeodrPhongIO io, const float *albedo,
-                                                             const double *lights, double *lights_b, Scratch *s) {
+                                                             const double *lights, double *lights_b, Scratch *s,
+                                                             const float *vis = nullptr) {
     constexpr int K = 3 + P;
     const double *lj = lights + blockIdx.x * K;
     double acc[K];
@@ -1251,10 +1273,17 @@ __global__ void __launch_bounds__(NT) k_point_lights_pixel_b(DeodrPhongIO io, co
             alpha += gA[c] * lj[3 + c];
             beta += gs[c] * lj[3 + c];
         }
+        double vj = 1.0;
+        if constexpr (VIS) {
+            vj = vis[p * gridDim.x + blockIdx.x];
+            alpha = __dmul_rn(alpha, vj);
+            beta = __dmul_rn(beta, vj);
+        }
         point_term_b(pt, n, alpha, beta, a * ks, e, n_b, d_b, v_b, q, e_b);
         for (int k = 0; k < 3; k++) acc[k] += d_b[k];
+        const double diff = VIS ? __dmul_rn(pt.diff, vj) : pt.diff, spec = VIS ? __dmul_rn(pt.spec, vj) : pt.spec;
 #pragma unroll
-        for (int c = 0; c < P; c++) acc[3 + c] += gA[c] * pt.diff + gs[c] * pt.spec;
+        for (int c = 0; c < P; c++) acc[3 + c] += gA[c] * diff + gs[c] * spec;
     }
     grid_sum_rows<K>(acc, s, lights_b);
 }
@@ -1373,18 +1402,20 @@ dim3 light_grid(long long items, int L, int P) {
     return dim3(L, std::max(1, std::min(reduce_grid(items), MAX_K * MAX_CTAS / (L * (3 + P)))));
 }
 
-template <int S, int P, bool SPLIT>
+template <int S, int P, bool SPLIT, bool VIS = false>
 void launch_point_phong_b(const DeodrPhongIO &io, const float *albedo, float *albedo_b, const double *sh,
-                          double *sh_b, const double *lights, int L, double *lights_b, Scratch *s, cudaStream_t st) {
+                          double *sh_b, const double *lights, int L, double *lights_b, Scratch *s, cudaStream_t st,
+                          const float *vis = nullptr, float *vis_b = nullptr) {
     const long long pixels = (long long)io.H * io.W;
     const int g = reduce_grid(pixels);
     if (io.camera_center_b)
-        k_phong_shade_b<true, S, SPLIT, P><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L);
+        k_phong_shade_b<true, S, SPLIT, P, VIS><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis, vis_b);
     else
-        k_phong_shade_b<false, S, SPLIT, P><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L);
+        k_phong_shade_b<false, S, SPLIT, P, VIS><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis, vis_b);
     if constexpr (S > 0)
         k_phong_sh_b<S, SPLIT><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo);
-    k_point_lights_pixel_b<P, SPLIT><<<light_grid(pixels, L, P), NT, 0, st>>>(io, albedo, lights, lights_b, s);
+    k_point_lights_pixel_b<P, SPLIT, VIS><<<light_grid(pixels, L, P), NT, 0, st>>>(io, albedo, lights, lights_b, s,
+                                                                                   vis);
 }
 
 }  // namespace
@@ -1781,6 +1812,56 @@ int deodr_b200_point_phong_shade_b(const DeodrPhongIO *io, const float *albedo, 
             launch_point_phong_b<S, P, true>(*io, albedo, albedo_b, sh, sh_b, lights, nb_lights, lights_b, s, st);
         else
             launch_point_phong_b<S, P, false>(*io, nullptr, nullptr, sh, sh_b, lights, nb_lights, lights_b, s, st);
+    });
+    return check_launch();
+}
+
+int deodr_b200_point_phong_shade_shadowed(const DeodrPhongIO *io, const float *albedo, const double *sh,
+                                          int sh_channels, const double *lights, int nb_lights, int light_channels,
+                                          const float *vis, void *stream) {
+    if (!phong_io_ok(io, albedo != nullptr) || !io->image || (!sh && sh_channels != 0) || !lights || !vis)
+        return bad("point_phong_shade_shadowed: bad argument (H, W >= 1, C in [1, 32760], offsets tiling [0, C + 7), "
+                   "or [0, 7) with off_albedo -1 and an albedo, channels, params, camera_center, background, image, "
+                   "lights and vis non-NULL, sh NULL only with sh_channels 0)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) || !light_channels_ok(light_channels, io->C) || nb_lights < 1 ||
+        nb_lights > MAX_LIGHTS)
+        return set_error(DEODR_B200_EUNSUPPORTED, "point_phong_shade_shadowed: nb_lights must be 1 to 8, and "
+                                                  "sh_channels and light_channels 1, or C from 1 to 4");
+    const int g = grid_of((long long)io->H * io->W);
+    cudaStream_t st = (cudaStream_t)stream;
+    with_point_channels(sh ? sh_channels : 0, light_channels, [&](auto S, auto P) {
+        if (albedo)
+            k_phong_shade<S, true, P, true><<<g, NT, 0, st>>>(*io, sh, albedo, lights, nb_lights, vis);
+        else
+            k_phong_shade<S, false, P, true><<<g, NT, 0, st>>>(*io, sh, nullptr, lights, nb_lights, vis);
+    });
+    return check_launch();
+}
+
+int deodr_b200_point_phong_shade_shadowed_b(const DeodrPhongIO *io, const float *albedo, float *albedo_b,
+                                            const double *sh, int sh_channels, double *sh_b, const double *lights,
+                                            int nb_lights, int light_channels, double *lights_b, const float *vis,
+                                            float *vis_b, double *scratch, void *stream) {
+    if (!phong_io_ok(io, albedo != nullptr) || !io->image_b || !io->channels_b || !io->params_b ||
+        (albedo && !albedo_b) || (!sh && sh_channels != 0) || (sh && !sh_b) || !lights || !lights_b || !vis ||
+        !vis_b || !scratch)
+        return bad("point_phong_shade_shadowed_b: bad argument (H, W >= 1, C in [1, 32760], offsets tiling [0, C + 7), "
+                   "or [0, 7) with off_albedo -1 and an albedo, channels, params, camera_center, background, image_b, "
+                   "channels_b, params_b, lights, lights_b, vis, vis_b and scratch non-NULL, albedo_b non-NULL with an "
+                   "albedo, sh NULL only with sh_channels 0, sh_b non-NULL with sh)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) || !light_channels_ok(light_channels, io->C) || nb_lights < 1 ||
+        nb_lights > MAX_LIGHTS)
+        return set_error(DEODR_B200_EUNSUPPORTED, "point_phong_shade_shadowed_b: nb_lights must be 1 to 8, and "
+                                                  "sh_channels and light_channels 1, or C from 1 to 4");
+    Scratch *s = reinterpret_cast<Scratch *>(scratch);
+    cudaStream_t st = (cudaStream_t)stream;
+    with_point_channels(sh ? sh_channels : 0, light_channels, [&](auto S, auto P) {
+        if (albedo)
+            launch_point_phong_b<S, P, true, true>(*io, albedo, albedo_b, sh, sh_b, lights, nb_lights, lights_b, s, st,
+                                                   vis, vis_b);
+        else
+            launch_point_phong_b<S, P, false, true>(*io, nullptr, nullptr, sh, sh_b, lights, nb_lights, lights_b, s,
+                                                    st, vis, vis_b);
     });
     return check_launch();
 }

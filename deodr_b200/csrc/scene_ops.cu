@@ -12,7 +12,9 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
+#include <type_traits>
 
 #include "../../include/deodr_b200.h"
 #include "reduce.cuh"
@@ -240,6 +242,235 @@ __global__ void __launch_bounds__(NT) k_project_camera_b(const double *points, i
                 x = tot[k - 3];
             camera_b[k] = x;
         }
+}
+
+// ---- cube shadow maps (the model of the shadow entry points, include/deodr_b200.h) --------------------------------
+
+constexpr int SHADOW_MAX_LIGHTS = 8;
+
+// the rows of R_k for the faces +x, -x, +y, -y, +z, -z: each a proper rotation (x_c cross y_c = z_c)
+__constant__ signed char CUBE_R[6][9] = {
+    {0, 1, 0, 0, 0, 1, 1, 0, 0},  {0, 0, 1, 0, 1, 0, -1, 0, 0}, {0, 0, 1, 1, 0, 0, 0, 1, 0},
+    {1, 0, 0, 0, 0, 1, 0, -1, 0}, {1, 0, 0, 0, 1, 0, 0, 0, 1},  {0, 1, 0, 1, 0, 0, 0, 0, -1}};
+
+// The camera vector [26] of face k of the cube around p: t = -R_k p is exact (one non-zero product of +-1 per row).
+__device__ __forceinline__ void cube_camera(const double *p, int k, int M, double v[26]) {
+    for (int i = 0; i < 3; i++) {
+        const double r0 = CUBE_R[k][3 * i], r1 = CUBE_R[k][3 * i + 1], r2 = CUBE_R[k][3 * i + 2];
+        v[4 * i] = r0;
+        v[4 * i + 1] = r1;
+        v[4 * i + 2] = r2;
+        v[4 * i + 3] = -(r0 * p[0] + r1 * p[1] + r2 * p[2]);
+    }
+    const double phi = 0.5 * M - 2.0, c = 0.5 * (M - 1);
+    v[12] = phi; v[13] = 0; v[14] = c;
+    v[15] = 0; v[16] = phi; v[17] = c;
+    v[18] = 0; v[19] = 0; v[20] = 1;
+    for (int i = 21; i < 26; i++) v[i] = 0;
+}
+
+__global__ void k_cube_cameras(const double *lights, int L, int stride, int M, double *cameras) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 6 * L) return;
+    cube_camera(lights + (i / 6) * stride, i % 6, M, cameras + 26 * i);
+}
+
+// k_project_dev for every face: item i = f n + vertex; the same project_point of the same camera values
+__global__ void k_cube_project(const double *points, int n, const double *cameras, long long items, int distorted,
+                               double *ij, double *depths) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= items) return;
+    const long long f = i / n, v = i - f * n;
+    project_point(load_cam(cameras + 26 * f, distorted), points + 3 * v, ij + 2 * i, depths + i);
+}
+
+// The cube projection's adjoint: one thread per vertex adds its 6L faces in order into points_b (no atomics); light
+// j's position receives -sum over its faces and vertices of R_k^T pc_b (t = -R_k p), summed with grid_sum.  A face
+// whose upstream gradients are exactly 0 adds nothing (a vertex at depth 0 would add 0 * inf = NaN).
+template <int L>
+__global__ void __launch_bounds__(NT) k_cube_project_b(const double *points, int n, const double *cameras,
+                                                       const float *ij_b, const float *depths_b, double *points_b,
+                                                       double *lights_b, int stride, Scratch *s) {
+    constexpr int K = 3 * L;
+    __shared__ double tot[K];
+    double acc[K];
+#pragma unroll
+    for (int k = 0; k < K; k++) acc[k] = 0;
+    for (long long i = (long long)blockIdx.x * NT + threadIdx.x; i < n; i += (long long)gridDim.x * NT) {
+        const double p[3] = {points[3 * i], points[3 * i + 1], points[3 * i + 2]};
+        double sum[3] = {0, 0, 0};
+#pragma unroll
+        for (int j = 0; j < L; j++)
+            for (int k = 0; k < 6; k++) {
+                const long long f = 6 * j + k, e = f * n + i;
+                const double gi = ij_b[2 * e], gj = ij_b[2 * e + 1], gd = depths_b[e];
+                if (gi == 0.0 && gj == 0.0 && gd == 0.0) continue;
+                PointAdjoint a;
+                double v[3];
+                project_point_b(load_cam(cameras + 26 * f, 0), p, gi, gj, &gd, 0, a, v);
+                for (int c = 0; c < 3; c++) {
+                    sum[c] = DADD(sum[c], v[c]);
+                    acc[3 * j + c] -= v[c];
+                }
+            }
+        for (int c = 0; c < 3; c++) points_b[3 * i + c] = DADD(points_b[3 * i + c], sum[c]);
+    }
+    if (grid_sum<K>(acc, s, tot))
+        for (int k = threadIdx.x; k < K; k += NT) lights_b[(k / 3) * stride + k % 3] += tot[k];
+}
+
+// The lookup of one surface point x in light p's cube map, kept for the adjoint.  valid: the projection is in front of
+// the face and finite (else V = 1).
+struct ShadowTap {
+    double cam[26], u, v, z, fu, fv, s[4], ds[4], top, bottom;
+    long long tap[4];  // texel indices into the light's six maps, taps 00, 10, 01, 11
+    bool valid;
+};
+
+__device__ __forceinline__ double shadow_lookup(const double x[3], const double *p, int M, const float *maps,
+                                                double bias, double softness, ShadowTap &t) {
+    const double d[3] = {x[0] - p[0], x[1] - p[1], x[2] - p[2]};
+    const double ax = fabs(d[0]), ay = fabs(d[1]), az = fabs(d[2]);
+    const int axis = ax >= ay && ax >= az ? 0 : (ay >= az ? 1 : 2);
+    const double da = axis == 0 ? d[0] : (axis == 1 ? d[1] : d[2]);  // selects, not an indexed (local) array
+    const int k = 2 * axis + (da > 0 ? 0 : 1);
+    cube_camera(p, k, M, t.cam);
+    double ij[2];
+    project_point(load_cam(t.cam, 0), x, ij, &t.z);
+    t.u = ij[0];
+    t.v = ij[1];
+    t.valid = t.z > 0 && isfinite(t.u) && isfinite(t.v);
+    if (!t.valid) return 1.0;
+    const double u0 = floor(t.u), v0 = floor(t.v), top = M - 1.0;
+    t.fu = t.u - u0;
+    t.fv = t.v - v0;
+    const long long c0 = (long long)fmin(fmax(u0, 0.0), top), c1 = (long long)fmin(fmax(u0 + 1, 0.0), top);
+    const long long r0 = (long long)fmin(fmax(v0, 0.0), top), r1 = (long long)fmin(fmax(v0 + 1, 0.0), top);
+    const long long face = (long long)k * M * M;
+    t.tap[0] = face + r0 * M + c0;
+    t.tap[1] = face + r0 * M + c1;
+    t.tap[2] = face + r1 * M + c0;
+    t.tap[3] = face + r1 * M + c1;
+    for (int q = 0; q < 4; q++) {
+        const double y = (((double)maps[t.tap[q]] + bias) - t.z) / softness + 1.0;
+        const double yc = fmin(fmax(y, 0.0), 1.0);
+        t.s[q] = yc * yc * (3.0 - 2.0 * yc);
+        t.ds[q] = y > 0.0 && y < 1.0 ? 6.0 * yc * (1.0 - yc) : 0.0;
+    }
+    t.top = t.s[0] + t.fu * (t.s[1] - t.s[0]);
+    t.bottom = t.s[2] + t.fu * (t.s[3] - t.s[2]);
+    return t.top + t.fv * (t.bottom - t.top);
+}
+
+// vis [H,W,L] of the G-buffer's pixels, one thread per pixel (1 where a = 0)
+__global__ void __launch_bounds__(NT) k_shadow_visibility(const float *ch, long long pixels, int stride, int off_pos,
+                                                          int off_cov, const double *lights, int L, int lstride,
+                                                          const float *maps, int M, double bias, double softness,
+                                                          float *vis) {
+    const long long p = (long long)blockIdx.x * NT + threadIdx.x;
+    if (p >= pixels) return;
+    const float *px = ch + p * stride;
+    const double a = px[off_cov];
+    float *out = vis + p * L;
+    if (a == 0.0) {
+        for (int j = 0; j < L; j++) out[j] = 1.0f;
+        return;
+    }
+    const double x[3] = {px[off_pos] / a, px[off_pos + 1] / a, px[off_pos + 2] / a};
+    for (int j = 0; j < L; j++) {
+        ShadowTap t;
+        out[j] = (float)shadow_lookup(x, lights + j * lstride, M, maps + (long long)6 * j * M * M, bias, softness, t);
+    }
+}
+
+// The visibility's adjoint from vis_b: per pixel and light the taps' gradients (maps_b, fp32 atomics) and x's, which
+// goes into the position and coverage slices of ch_b (accumulated) and, negated, into the light's position (summed
+// with grid_sum in a fixed order and added to lights_b).
+template <int L>
+__global__ void __launch_bounds__(NT) k_shadow_visibility_b(const float *ch, float *ch_b, long long pixels, int stride,
+                                                            int off_pos, int off_cov, const double *lights,
+                                                            int lstride, const float *maps, int M, double bias,
+                                                            double softness, const float *vis_b, float *maps_b,
+                                                            double *lights_b, Scratch *s) {
+    constexpr int K = 3 * L;
+    __shared__ double tot[K];
+    double acc[K];
+#pragma unroll
+    for (int k = 0; k < K; k++) acc[k] = 0;
+    for (long long p = (long long)blockIdx.x * NT + threadIdx.x; p < pixels; p += (long long)gridDim.x * NT) {
+        const float *px = ch + p * stride;
+        const double a = px[off_cov];
+        if (a == 0.0) continue;
+        const double x[3] = {px[off_pos] / a, px[off_pos + 1] / a, px[off_pos + 2] / a};
+        double x_b[3] = {0, 0, 0};
+#pragma unroll
+        for (int j = 0; j < L; j++) {
+            const double g = vis_b[p * L + j];
+            if (g == 0.0) continue;
+            ShadowTap t;
+            shadow_lookup(x, lights + j * lstride, M, maps + (long long)6 * j * M * M, bias, softness, t);
+            if (!t.valid) continue;
+            // V = top + fv (bottom - top), top / bottom = lerps in fu of the taps 00, 10 / 01, 11
+            const double top_b = g * (1.0 - t.fv), bottom_b = g * t.fv;
+            const double fv_b = g * (t.bottom - t.top);
+            const double fu_b = top_b * (t.s[1] - t.s[0]) + bottom_b * (t.s[3] - t.s[2]);
+            const double s_b[4] = {top_b * (1.0 - t.fu), top_b * t.fu, bottom_b * (1.0 - t.fu), bottom_b * t.fu};
+            double z_b = 0;
+            float *mb = maps_b + (long long)6 * j * M * M;
+            for (int q = 0; q < 4; q++) {
+                const double D_b = s_b[q] * t.ds[q] / softness;
+                if (D_b != 0.0) atomicAdd(mb + t.tap[q], (float)D_b);
+                z_b -= D_b;
+            }
+            PointAdjoint pa;
+            double v[3];
+            project_point_b(load_cam(t.cam, 0), x, fu_b, fv_b, &z_b, 0, pa, v);
+            for (int c = 0; c < 3; c++) {
+                x_b[c] += v[c];
+                acc[3 * j + c] -= v[c];
+            }
+        }
+        float *pb = ch_b + p * stride;
+        for (int c = 0; c < 3; c++) pb[off_pos + c] = (float)((double)pb[off_pos + c] + x_b[c] / a);
+        pb[off_cov] = (float)((double)pb[off_cov] - ((x_b[0] * x[0] + x_b[1] * x[1]) + x_b[2] * x[2]) / a);
+    }
+    if (grid_sum<K>(acc, s, tot))
+        for (int k = threadIdx.x; k < K; k += NT) lights_b[(k / 3) * lstride + k % 3] += tot[k];
+}
+
+// Calls f(L) with L from 1 to SHADOW_MAX_LIGHTS as a compile-time constant
+template <typename F>
+void with_lights(int L, F &&f) {
+    switch (L) {
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 2: return f(std::integral_constant<int, 2>{});
+        case 3: return f(std::integral_constant<int, 3>{});
+        case 4: return f(std::integral_constant<int, 4>{});
+        case 5: return f(std::integral_constant<int, 5>{});
+        case 6: return f(std::integral_constant<int, 6>{});
+        case 7: return f(std::integral_constant<int, 7>{});
+        default: return f(std::integral_constant<int, 8>{});
+    }
+}
+
+// grid_sum of K sums: at most MAX_CTAS CTAs, and beyond MAX_K sums at most MAX_K * MAX_CTAS / K
+int sum_grid(long long items, int K) {
+    const long long g = std::max<long long>(1, (items + NT - 1) / NT);
+    return (int)std::min<long long>(g, K <= MAX_K ? MAX_CTAS : MAX_K * MAX_CTAS / K);
+}
+
+bool shadow_map_ok(int M) { return M >= 8 && M <= 4096; }
+bool shadow_band_ok(double bias, double softness) {
+    return std::isfinite(bias) && std::isfinite(softness) && bias > 0 && softness > 0;
+}
+bool shadow_lights_ok(int L, int P) { return L >= 1 && L <= SHADOW_MAX_LIGHTS && P >= 1 && P <= 4; }
+
+// the G-buffer sizes and the position and coverage offsets the lookup reads, in either Phong form
+bool shadow_io_ok(const DeodrPhongIO *io) {
+    if (!io || !io->channels || io->H < 1 || io->W < 1 || io->C < 1 || io->C > 32760) return false;
+    const int K = io->off_albedo == -1 ? 7 : io->C + 7;
+    return io->off_position >= 0 && io->off_position <= K - 3 && io->off_coverage >= 0 && io->off_coverage < K &&
+           (io->off_coverage < io->off_position || io->off_coverage >= io->off_position + 3);
 }
 
 struct Light {
@@ -569,6 +800,82 @@ int deodr_b200_vertex_normals_b(const DeodrMeshTopology *mesh, const double *ver
     cudaStream_t st = (cudaStream_t)stream;
     k_vertex_normals_b1<<<grid_of(mesh->nb_vertices), BLOCK, 0, st>>>(*mesh, vertices, vertex_normals_b, vertex_scratch);
     k_face_normals_b<<<grid_of(mesh->nb_faces), BLOCK, 0, st>>>(*mesh, vertices, vertex_scratch, nullptr, vertices_b);
+    return check_launch();
+}
+
+int deodr_b200_cube_project(const double *vertices, int n, const double *lights, int nb_lights, int light_channels,
+                            int map_size, double *cameras, double *ij, double *depths, void *stream) {
+    if (n < 1 || !vertices || !lights || !cameras || !ij || !depths || !shadow_map_ok(map_size))
+        return set_error(DEODR_B200_EINVAL, "cube_project: bad argument (n >= 1, every pointer non-NULL, map_size in "
+                                            "[8, 4096])");
+    if (!shadow_lights_ok(nb_lights, light_channels))
+        return set_error(DEODR_B200_EUNSUPPORTED, "cube_project: nb_lights must be 1 to 8 and light_channels 1 to 4");
+    cudaStream_t st = (cudaStream_t)stream;
+    k_cube_cameras<<<1, 6 * SHADOW_MAX_LIGHTS, 0, st>>>(lights, nb_lights, 3 + light_channels, map_size, cameras);
+    const long long items = 6LL * nb_lights * n;
+    k_cube_project<<<(unsigned)((items + BLOCK - 1) / BLOCK), BLOCK, 0, st>>>(vertices, n, cameras, items, 0, ij,
+                                                                            depths);
+    return check_launch();
+}
+
+int deodr_b200_cube_project_b(const double *vertices, int n, const double *lights, int nb_lights, int light_channels,
+                              int map_size, const double *cameras, const float *ij_b, const float *depths_b,
+                              double *vertices_b, double *lights_b, double *scratch, void *stream) {
+    if (n < 1 || !vertices || !lights || !cameras || !ij_b || !depths_b || !vertices_b || !lights_b || !scratch ||
+        !shadow_map_ok(map_size))
+        return set_error(DEODR_B200_EINVAL, "cube_project_b: bad argument (n >= 1, every pointer non-NULL, map_size "
+                                            "in [8, 4096])");
+    if (!shadow_lights_ok(nb_lights, light_channels))
+        return set_error(DEODR_B200_EUNSUPPORTED, "cube_project_b: nb_lights must be 1 to 8 and light_channels 1 to 4");
+    cudaStream_t st = (cudaStream_t)stream;
+    Scratch *s = reinterpret_cast<Scratch *>(scratch);
+    with_lights(nb_lights, [&](auto L) {
+        k_cube_project_b<L><<<sum_grid(n, 3 * L), NT, 0, st>>>(vertices, n, cameras, ij_b, depths_b, vertices_b,
+                                                               lights_b, 3 + light_channels, s);
+    });
+    return check_launch();
+}
+
+int deodr_b200_shadow_visibility(const DeodrPhongIO *io, const double *lights, int nb_lights, int light_channels,
+                                 const float *maps, int map_size, double bias, double softness, float *vis,
+                                 void *stream) {
+    if (!shadow_io_ok(io) || !lights || !maps || !vis || !shadow_map_ok(map_size) || !shadow_band_ok(bias, softness))
+        return set_error(DEODR_B200_EINVAL, "shadow_visibility: bad argument (H, W >= 1, C in [1, 32760], position and "
+                                            "coverage offsets inside the G-buffer, every pointer non-NULL, map_size in "
+                                            "[8, 4096], bias and softness finite and > 0)");
+    if (nb_lights < 1 || nb_lights > SHADOW_MAX_LIGHTS || !(light_channels == 1 || (light_channels == io->C &&
+                                                                                    io->C >= 2 && io->C <= 4)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "shadow_visibility: nb_lights must be 1 to 8, and light_channels 1, "
+                                                  "or C from 1 to 4");
+    const long long pixels = (long long)io->H * io->W;
+    const int stride = io->off_albedo == -1 ? 7 : io->C + 7;
+    k_shadow_visibility<<<(unsigned)((pixels + NT - 1) / NT), NT, 0, (cudaStream_t)stream>>>(
+        io->channels, pixels, stride, io->off_position, io->off_coverage, lights, nb_lights, 3 + light_channels, maps,
+        map_size, bias, softness, vis);
+    return check_launch();
+}
+
+int deodr_b200_shadow_visibility_b(const DeodrPhongIO *io, const double *lights, int nb_lights, int light_channels,
+                                   const float *maps, int map_size, double bias, double softness, const float *vis_b,
+                                   float *maps_b, double *lights_b, double *scratch, void *stream) {
+    if (!shadow_io_ok(io) || !io->channels_b || !lights || !maps || !vis_b || !maps_b || !lights_b || !scratch ||
+        !shadow_map_ok(map_size) || !shadow_band_ok(bias, softness))
+        return set_error(DEODR_B200_EINVAL, "shadow_visibility_b: bad argument (H, W >= 1, C in [1, 32760], position "
+                                            "and coverage offsets inside the G-buffer, every pointer non-NULL, "
+                                            "map_size in [8, 4096], bias and softness finite and > 0)");
+    if (nb_lights < 1 || nb_lights > SHADOW_MAX_LIGHTS || !(light_channels == 1 || (light_channels == io->C &&
+                                                                                    io->C >= 2 && io->C <= 4)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "shadow_visibility_b: nb_lights must be 1 to 8, and light_channels "
+                                                  "1, or C from 1 to 4");
+    const long long pixels = (long long)io->H * io->W;
+    const int stride = io->off_albedo == -1 ? 7 : io->C + 7;
+    cudaStream_t st = (cudaStream_t)stream;
+    Scratch *s = reinterpret_cast<Scratch *>(scratch);
+    with_lights(nb_lights, [&](auto L) {
+        k_shadow_visibility_b<L><<<sum_grid(pixels, 3 * L), NT, 0, st>>>(
+            io->channels, io->channels_b, pixels, stride, io->off_position, io->off_coverage, lights,
+            3 + light_channels, maps, map_size, bias, softness, vis_b, maps_b, lights_b, s);
+    });
     return check_launch();
 }
 

@@ -12,6 +12,7 @@ PyTorch is used for device memory and streams only.
 
 from __future__ import annotations
 
+import copy
 import ctypes as C
 from typing import Dict, Optional, Sequence, Tuple
 
@@ -424,7 +425,8 @@ def _phong_io(channels: torch.Tensor, params: torch.Tensor, center: torch.Tensor
 
 def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: torch.Tensor,
                 background: torch.Tensor, sh: Optional[torch.Tensor] = None,
-                albedo: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None) -> torch.Tensor:
+                albedo: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None,
+                visibility: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The per-pixel shading of a G-buffer (deodr_b200_phong_shade, or deodr_b200_sh_phong_shade with ``sh``; model in
     include/deodr_b200.h): ``channels``
     [H,W,C+7] f32 laid out (albedo C, normal 3, position 3, coverage 1), ``params`` [6] fp64 on the device = (light
@@ -432,12 +434,23 @@ def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: tor
     ``background`` [C] -> image [H,W,C] f32.  ``sh``: an optional spherical-harmonics environment [9] or [9,C] fp64
     on the device.  ``albedo``: the albedo [H,W,C] f32 as a raster of its own (a textured mesh's), with ``channels``
     then [H,W,7] = (normal, position, coverage) (deodr_b200_phong_shade_albedo).  ``point_lights``: a point-light
-    table [L, 3 + S] fp64 on the device, in either form (deodr_b200_point_phong_shade)."""
+    table [L, 3 + S] fp64 on the device, in either form (deodr_b200_point_phong_shade).  ``visibility``: with point
+    lights, the lights' visibility [H,W,L] f32 (:func:`shadow_visibility`), which multiplies each light's diffuse and
+    specular terms (deodr_b200_point_phong_shade_shadowed)."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     H, W = keep[0].shape[:2]
     image = torch.empty((H, W, io.C), dtype=torch.float32, device=keep[0].device)
     io.image = image.data_ptr()
-    if point_lights is not None:
+    if visibility is not None:
+        if point_lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        lights, L, P = _check_point_lights(point_lights, image.device)
+        vis = _check_visibility(visibility, H, W, L, image.device)
+        sh, S = _check_sh(sh, image.device) if sh is not None else (None, 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        _cabi.check(_cabi.load().deodr_b200_point_phong_shade_shadowed(
+            C.byref(io), ptr(keep[4]), ptr(sh), S, lights.data_ptr(), L, P, vis.data_ptr(), _stream(image.device)))
+    elif point_lights is not None:
         lights, L, P = _check_point_lights(point_lights, image.device)
         sh, S = _check_sh(sh, image.device) if sh is not None else (None, 0)
         ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
@@ -461,7 +474,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
                          background: torch.Tensor, image_b: torch.Tensor, scratch: torch.Tensor,
                          center_grad: bool = False, sh: Optional[torch.Tensor] = None,
                          albedo: Optional[torch.Tensor] = None,
-                         point_lights: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
+                         point_lights: Optional[torch.Tensor] = None,
+                         visibility: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
     """-> (channels_b [H,W,C+7] f32, params_b [6] fp64), the adjoint of :func:`phong_shade` from ``image_b`` [H,W,C]
     (deodr_b200_phong_shade_b, or deodr_b200_sh_phong_shade_b with ``sh``).  channels_b includes the coverage channel's gradient; ``params_b`` is summed over the
     pixels in a fixed order (bit-reproducible).  ``scratch``: a buffer of ``mesh_fitter.new_scratch``.  With
@@ -469,7 +483,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     it then holds sh_b, shaped like ``sh``, also summed in a fixed order.  With a separate ``albedo`` (see
     :func:`phong_shade`; channels_b is then [H,W,7]) the result ends with albedo_b [H,W,C] f32
     (deodr_b200_phong_shade_albedo_b).  With ``point_lights`` the result ends with lights_b [L, 3 + S] fp64, summed
-    in a fixed order (deodr_b200_point_phong_shade_b)."""
+    in a fixed order (deodr_b200_point_phong_shade_b); with ``visibility`` too it then ends with vis_b [H,W,L] f32
+    (deodr_b200_point_phong_shade_shadowed_b)."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     dev = keep[0].device
     S = _check_sh(sh, dev)[1] if sh is not None else 0
@@ -488,8 +503,18 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
     if albedo is not None:
         albedo_b = torch.empty((H, W, io.C), dtype=torch.float32, device=dev)
-    lights_b = None
-    if point_lights is not None:
+    lights_b = vis_b = None
+    if visibility is not None:
+        if point_lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        lights, L, P = _check_point_lights(point_lights, dev)
+        vis = _check_visibility(visibility, H, W, L, dev)
+        lights_b = torch.empty_like(lights)
+        vis_b = torch.empty((H, W, L), dtype=torch.float32, device=dev)
+        _cabi.check(_cabi.load().deodr_b200_point_phong_shade_shadowed_b(
+            C.byref(io), ptr(keep[4]), ptr(albedo_b), ptr(sh), S, ptr(sh_b), lights.data_ptr(), L, P,
+            lights_b.data_ptr(), vis.data_ptr(), vis_b.data_ptr(), scratch.data_ptr(), _stream(dev)))
+    elif point_lights is not None:
         lights, L, P = _check_point_lights(point_lights, dev)
         lights_b = torch.empty_like(lights)
         _cabi.check(_cabi.load().deodr_b200_point_phong_shade_b(
@@ -508,7 +533,140 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     out = (channels_b, params_b) if center_b is None else (channels_b, params_b, center_b)
     out = out if sh_b is None else out + (sh_b,)
     out = out if albedo_b is None else out + (albedo_b,)
-    return out if lights_b is None else out + (lights_b,)
+    out = out if lights_b is None else out + (lights_b,)
+    return out if vis_b is None else out + (vis_b,)
+
+
+# ---- shadows from point lights (the model in include/deodr_b200.h) ---------------------------------------------------
+
+SHADOW_FAR = 1e30  # DEODR_B200_SHADOW_FAR: the background depth of the cube shadow maps
+
+
+def _check_visibility(vis: torch.Tensor, H: int, W: int, L: int, device) -> torch.Tensor:
+    if not isinstance(vis, torch.Tensor) or vis.dtype != torch.float32 or tuple(vis.shape) != (H, W, L) \
+            or not vis.is_contiguous() or vis.device != torch.device(device):
+        raise ValueError(f"visibility must be a contiguous [{H},{W},{L}] f32 tensor on {device}; got "
+                         f"{getattr(vis, 'dtype', type(vis))} {tuple(getattr(vis, 'shape', ()))}")
+    return vis
+
+
+def _check_maps(maps: torch.Tensor, L: int, device) -> Tuple[torch.Tensor, int]:
+    """-> (maps, M) for cube maps [6L, M, M] f32, contiguous, on ``device``."""
+    if not isinstance(maps, torch.Tensor) or maps.dtype != torch.float32 or maps.dim() != 3 \
+            or maps.shape[0] != 6 * L or maps.shape[1] != maps.shape[2] or not maps.is_contiguous() \
+            or maps.device != torch.device(device):
+        raise ValueError(f"maps must be a contiguous [6L, M, M] f32 tensor on {device} with L = {L}; got "
+                         f"{getattr(maps, 'dtype', type(maps))} {tuple(getattr(maps, 'shape', ()))}")
+    return maps, maps.shape[1]
+
+
+def _shadow_io(channels: torch.Tensor, albedo: Optional[torch.Tensor]) -> Tuple[_cabi.PhongIO, torch.Tensor]:
+    """The G-buffer part of a ``DeodrPhongIO`` the visibility reads: [H,W,C+7] (albedo first), or [H,W,7] with a
+    separate ``albedo`` [H,W,C] (only its channel count is used)."""
+    channels = channels.to(dtype=torch.float32).contiguous()
+    if channels.dim() != 3 or channels.shape[2] < PHONG_EXTRA_CHANNELS + (0 if albedo is not None else 1) \
+            or (albedo is not None and channels.shape[2] != PHONG_EXTRA_CHANNELS):
+        raise ValueError(f"channels must be [H,W,C+7], or [H,W,7] with an albedo; got {tuple(channels.shape)}")
+    H, W, K = channels.shape
+    nc = K - PHONG_EXTRA_CHANNELS if albedo is None else albedo.shape[-1]
+    io = _cabi.PhongIO()
+    io.channels, io.H, io.W, io.C = channels.data_ptr(), H, W, nc
+    if albedo is None:
+        io.off_albedo, io.off_normal, io.off_position, io.off_coverage = 0, nc, nc + 3, nc + 6
+    else:
+        io.off_albedo, io.off_normal, io.off_position, io.off_coverage = -1, 0, 3, 6
+    return io, channels
+
+
+def cube_project(vertices: torch.Tensor, lights: torch.Tensor,
+                 map_size: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The cube cameras of the point lights ``lights`` [L, 3 + S] and the vertices [V,3] projected through them
+    (deodr_b200_cube_project) -> (cameras [6L, 26], ij [6L, V, 2], depths [6L, V]) fp64; face 6 j + k is light j's
+    +x, -x, +y, -y, +z or -z face.  Each face's ij and depths are bit-identical to :func:`project_points_dev` with its
+    camera vector."""
+    dev = vertices.device
+    vertices = _f64(vertices, dev)
+    lights, L, S = _check_point_lights(lights, dev)
+    n = vertices.shape[0]
+    cameras = torch.empty((6 * L, CAMERA_VECTOR_SIZE), dtype=torch.float64, device=dev)
+    ij = torch.empty((6 * L, n, 2), dtype=torch.float64, device=dev)
+    depths = torch.empty((6 * L, n), dtype=torch.float64, device=dev)
+    _cabi.check(_cabi.load().deodr_b200_cube_project(vertices.data_ptr(), n, lights.data_ptr(), L, S, int(map_size),
+                                                     cameras.data_ptr(), ij.data_ptr(), depths.data_ptr(),
+                                                     _stream(dev)))
+    return cameras, ij, depths
+
+
+def cube_project_backward(vertices: torch.Tensor, lights: torch.Tensor, map_size: int, cameras: torch.Tensor,
+                          ij_b: torch.Tensor, depths_b: torch.Tensor, scratch: torch.Tensor,
+                          vertices_b: Optional[torch.Tensor] = None,
+                          lights_b: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The adjoint of :func:`cube_project` from ``ij_b`` [6L, V, 2] and ``depths_b`` [6L, V] (fp32, the rasteriser's)
+    -> (vertices_b [V,3], lights_b [L, 3 + S]) fp64, accumulated into the given tensors (created zeroed if None):
+    every vertex adds its 6L faces in a fixed order, and the lights' positions their faces' share, summed in a fixed
+    order (deodr_b200_cube_project_b).  ``scratch``: a buffer of ``mesh_fitter.new_scratch``."""
+    dev = vertices.device
+    vertices = _f64(vertices, dev)
+    lights, L, S = _check_point_lights(lights, dev)
+    n = vertices.shape[0]
+    ij_b = ij_b.to(device=dev, dtype=torch.float32).contiguous()
+    depths_b = depths_b.to(device=dev, dtype=torch.float32).contiguous()
+    if tuple(ij_b.shape) != (6 * L, n, 2) or depths_b.numel() != 6 * L * n:
+        raise ValueError(f"ij_b must be [{6 * L},{n},2] and depths_b [{6 * L},{n}]; got {tuple(ij_b.shape)} and "
+                         f"{tuple(depths_b.shape)}")
+    if vertices_b is None:
+        vertices_b = torch.zeros((n, 3), dtype=torch.float64, device=dev)
+    if lights_b is None:
+        lights_b = torch.zeros_like(lights)
+    _cabi.check(_cabi.load().deodr_b200_cube_project_b(
+        vertices.data_ptr(), n, lights.data_ptr(), L, S, int(map_size), cameras.data_ptr(), ij_b.data_ptr(),
+        depths_b.data_ptr(), vertices_b.data_ptr(), lights_b.data_ptr(), scratch.data_ptr(), _stream(dev)))
+    return vertices_b, lights_b
+
+
+def shadow_visibility(channels: torch.Tensor, lights: torch.Tensor, maps: torch.Tensor, bias: float,
+                      softness: float, albedo: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The visibility [H,W,L] f32 of a Phong G-buffer's pixels (``channels`` [H,W,C+7], or [H,W,7] beside a separate
+    ``albedo``) under the point lights' cube shadow maps ``maps`` [6L, M, M] f32 (deodr_b200_shadow_visibility; the
+    model in include/deodr_b200.h): a 2x2 bilinear filter of smoothstep depth tests, ``bias`` and ``softness`` in
+    world units.  1 where the coverage is 0."""
+    dev = channels.device
+    io, channels = _shadow_io(channels, albedo)
+    lights, L, S = _check_point_lights(lights, dev)
+    maps, M = _check_maps(maps, L, dev)
+    vis = torch.empty((io.H, io.W, L), dtype=torch.float32, device=dev)
+    _cabi.check(_cabi.load().deodr_b200_shadow_visibility(C.byref(io), lights.data_ptr(), L, S, maps.data_ptr(), M,
+                                                          float(bias), float(softness), vis.data_ptr(),
+                                                          _stream(dev)))
+    return vis
+
+
+def shadow_visibility_backward(channels: torch.Tensor, lights: torch.Tensor, maps: torch.Tensor, bias: float,
+                               softness: float, vis_b: torch.Tensor, scratch: torch.Tensor,
+                               albedo: Optional[torch.Tensor] = None, channels_b: Optional[torch.Tensor] = None,
+                               maps_b: Optional[torch.Tensor] = None,
+                               lights_b: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
+    """The adjoint of :func:`shadow_visibility` from ``vis_b`` [H,W,L] -> (channels_b, maps_b [6L, M, M] f32,
+    lights_b [L, 3 + S] fp64), each accumulated into the given tensor (created zeroed if None): the position and
+    coverage slices of channels_b, the texels (fp32 atomics) and the lights' positions, summed in a fixed order
+    (deodr_b200_shadow_visibility_b).  ``scratch``: a buffer of ``mesh_fitter.new_scratch``."""
+    dev = channels.device
+    io, channels = _shadow_io(channels, albedo)
+    lights, L, S = _check_point_lights(lights, dev)
+    maps, M = _check_maps(maps, L, dev)
+    vis_b = _check_visibility(vis_b.to(dev, torch.float32).contiguous(), io.H, io.W, L, dev)
+    if channels_b is None:
+        channels_b = torch.zeros_like(channels)
+    if tuple(channels_b.shape) != tuple(channels.shape) or channels_b.dtype != torch.float32 \
+            or not channels_b.is_contiguous():
+        raise ValueError(f"channels_b must be a contiguous f32 tensor shaped like channels {tuple(channels.shape)}")
+    maps_b = torch.zeros_like(maps) if maps_b is None else maps_b
+    lights_b = torch.zeros_like(lights) if lights_b is None else lights_b
+    io.channels_b = channels_b.data_ptr()
+    _cabi.check(_cabi.load().deodr_b200_shadow_visibility_b(
+        C.byref(io), lights.data_ptr(), L, S, maps.data_ptr(), M, float(bias), float(softness), vis_b.data_ptr(),
+        maps_b.data_ptr(), lights_b.data_ptr(), scratch.data_ptr(), _stream(dev)))
+    return channels_b, maps_b, lights_b
 
 
 def _light(light_directional):
@@ -804,6 +962,111 @@ def loop_subdivision(faces, vertices, colors=None, n_iter: int = 1):
     return sub.faces, fv.cpu().numpy(), (fc.cpu().numpy() if fc is not None else None)
 
 
+SHADOW_MAP_SIZES = (8, 4096)
+
+
+def check_shadow_arguments(shading: str, point_lights, size: int, bias, softness) -> int:
+    """The refusals of a view's (or a scene's) shadow arguments -> the map size M (0: no shadows)."""
+    size = int(size)
+    if size == 0:
+        return 0
+    if shading not in ("phong", "phong_textured"):
+        raise ValueError("shadows need per-pixel shading (shading='phong' or 'phong_textured'): a shadow edge crosses "
+                         "triangles, and per-vertex visibility would smear it over each one")
+    if point_lights is None:
+        raise ValueError("shadows are cast from point lights: this view has none")
+    if not SHADOW_MAP_SIZES[0] <= size <= SHADOW_MAP_SIZES[1]:
+        raise ValueError(f"shadow_map_size must be 0 or lie in [{SHADOW_MAP_SIZES[0]}, {SHADOW_MAP_SIZES[1]}]; got {size}")
+    if bias is None or softness is None:
+        raise ValueError("shadows need both shadow_bias and shadow_softness (world units: no default is free of scale)")
+    if not (np.isfinite(bias) and np.isfinite(softness) and bias > 0 and softness > 0):
+        raise ValueError(f"shadow_bias and shadow_softness must be finite and > 0; got {bias} and {softness}")
+    return size
+
+
+class ShadowCubes:
+    """The cube shadow maps of L point lights: 6L one-channel depth scenes of a mesh (face 6 j + k), whose ij, depths,
+    colours (the depth) and silhouette flags are slices of one buffer each, filled by one projection launch
+    (:func:`cube_project`) and one silhouette launch over a topology of 6L disjoint copies of the faces.  The caller
+    renders :attr:`scenes` beside its own in one renderer call, with :meth:`outputs` as their results, and
+    back-propagates them in one call with :meth:`image_bs` and :meth:`grads`, then calls :meth:`backward`."""
+
+    def __init__(self, faces_u32: np.ndarray, V: int, L: int, M: int, clockwise: bool, device):
+        from .renderer import DeviceScene
+        from .scenes import SceneArrays
+
+        T, NF = faces_u32.shape[0], 6 * L
+        self.L, self.M, self.V, self.device = L, M, V, device
+        tiled = (faces_u32[None].astype(np.int64) + (np.arange(NF) * V)[:, None, None]).reshape(-1, 3)
+        self.topology = MeshTopology(tiled, NF * V, clockwise=clockwise, device=device)
+        self.edgeflags = torch.zeros((NF * T, 3), dtype=torch.uint8, device=device)
+        self.colors = torch.zeros((NF, V, 1), dtype=torch.float32, device=device)
+        self.ij_b = torch.zeros((NF, V, 2), dtype=torch.float32, device=device)
+        self.colors_b = torch.zeros((NF, V, 1), dtype=torch.float32, device=device)
+        self.maps4 = torch.empty((NF, M, M, 1), dtype=torch.float32, device=device)
+        self.maps = self.maps4.view(NF, M, M)
+        self.maps_b = torch.zeros((NF, M, M), dtype=torch.float32, device=device)
+        self.cameras = self.ij = self.depths = None
+        self.fwds = None
+        # a depth render (DeviceMeshView.render_depth) with culling on over the background depth SHADOW_FAR
+        base = DeviceScene(SceneArrays(
+            faces=faces_u32, faces_uv=np.zeros((T, 3), np.uint32), ij=np.zeros((V, 2)), depths=np.ones(V),
+            textured=np.zeros(T, bool), uv=np.zeros((1, 2)), shade=np.zeros(V), colors=np.zeros((V, 1)),
+            shaded=np.zeros(T, bool), edgeflags=np.zeros((T, 3), bool), height=M, width=M, nb_colors=1,
+            texture=np.zeros((2, 2, 1)), background_image=None, background_color=np.array([SHADOW_FAR]),
+            clockwise=clockwise, backface_culling=True, strict_edge=True, perspective_correct=False,
+            integer_pixel_centers=True), device)
+        self._base = base
+        self.scenes = []
+        for f in range(NF):
+            sc = copy.copy(base)
+            sc.t = dict(base.t)
+            sc.t.update(colors=self.colors[f], edgeflags=self.edgeflags[f * T:(f + 1) * T])
+            self.scenes.append(sc)
+        # the outputs of every face (the image a slice of the maps), and the shared gradient slots a depth scene
+        # never writes (no texture, no shade)
+        self._outputs = [{"image": self.maps4[f], "z_buffer": torch.empty((M, M), dtype=torch.float64, device=device),
+                          "owner": torch.empty((M, M), dtype=torch.int32, device=device), "face_id": None,
+                          "barycentric": None, "err_buffer": None} for f in range(NF)]
+        self._unused_b = base.zero_grads()
+
+    def prepare(self, vertices: torch.Tensor, lights: torch.Tensor) -> None:
+        """Projects the vertices through the cube cameras of ``lights`` (read on the device) and sets the scenes'
+        ij, depths, colours and silhouette flags."""
+        if lights.shape[0] != self.L:
+            raise ValueError(f"the view's shadow maps were made for {self.L} lights; the table has {lights.shape[0]}")
+        self.cameras, self.ij, self.depths = cube_project(vertices, lights, self.M)
+        self.colors.copy_(self.depths[:, :, None])
+        self.topology.edge_on_silhouette(self.ij.view(-1, 2), out=self.edgeflags)
+        for f, sc in enumerate(self.scenes):
+            sc.t["ij"], sc.t["depths"] = self.ij[f], self.depths[f]
+
+    def outputs(self):
+        return self._outputs
+
+    def zero_maps_b(self) -> torch.Tensor:
+        self.maps_b.zero_()
+        return self.maps_b
+
+    def image_bs(self, maps_b: torch.Tensor):
+        return [maps_b[f].view(self.M, self.M, 1) for f in range(6 * self.L)]
+
+    def grads(self):
+        """The faces' gradient slots: ij_b and colors_b slices of one buffer each, zeroed."""
+        self.ij_b.zero_()
+        self.colors_b.zero_()
+        u = self._unused_b
+        return [{"ij_b": self.ij_b[f], "colors_b": self.colors_b[f], "uv_b": u["uv_b"], "shade_b": u["shade_b"],
+                 "texture_b": u["texture_b"]} for f in range(6 * self.L)]
+
+    def backward(self, vertices: torch.Tensor, lights: torch.Tensor, vertices_b: torch.Tensor,
+                 lights_b: torch.Tensor, scratch: torch.Tensor) -> None:
+        """The cube projection's adjoint after the faces' raster adjoint: depths_b = colors_b (the colour is the
+        depth), accumulated into vertices_b and the positions of lights_b."""
+        cube_project_backward(vertices, lights, self.M, self.cameras, self.ij_b, self.colors_b.view(6 * self.L, -1),
+                              scratch, vertices_b=vertices_b, lights_b=lights_b)
+
+
 class DeviceMeshView:
     """One view of a lit mesh (Gouraud by default), device-resident end to end: the chain of ``Scene3D.render`` /
     ``render_backward`` (deodr/differentiable_renderer.py:871-1052) with every step on the GPU -
@@ -854,14 +1117,26 @@ class DeviceMeshView:
     to 4), L from 1 to 8.  It is read at every render, so a fit can update it in place.  Every shading uses it,
     textured Gouraud views grey lights only; :meth:`backward` then also returns ``point_lights_b``, shaped like the
     table and summed in a fixed order, and a Gouraud view adds the lights' share of the vertex positions into
-    ``vertices_b``.  Depth and deferred renders ignore it."""
+    ``vertices_b``.  Depth and deferred renders ignore it.
+
+    ``shadow_map_size`` M > 0 makes the point lights cast shadows in a Phong or textured Phong view (the model in
+    include/deodr_b200.h): every light gets a cube of six M x M depth maps of the mesh, rendered with the view's sigma
+    in map pixels, and each pixel's light terms are multiplied by a soft 2x2 depth test against them,
+    ``shadow_bias`` and ``shadow_softness`` (world units, both required) setting where it starts and how wide it is.
+    The view's raster(s) and the 6L cube faces are rendered by one renderer call and back-propagated by one, and
+    :meth:`backward` adds the shadows' share to ``vertices_b`` (occluders and receivers) and to the lights' positions
+    in ``point_lights_b``; the camera's gradient has none (the lookup does not read the camera).  Gouraud views refuse
+    shadows: a shadow edge crosses triangles, and per-vertex visibility would smear it over each one.
+    :meth:`shadow_maps` returns the last maps."""
 
     def __init__(self, faces, nb_vertices: int, camera, height: int, width: int, renderer=None,
                  light_directional=None, ambient: float = 1.0, background_color=(0.0, 0.0, 0.0), sigma: float = 1.0,
                  clockwise: bool = False, device="cuda", slot: int = 0, uv=None, faces_uv=None, texture=None,
                  backface_culling: bool = True, perspective_correct: bool = False, shading: str = "gouraud",
                  specular: float = 0.0, shininess: float = 16.0, has_distortion: bool = True,
-                 sh: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None):
+                 sh: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None,
+                 shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
+                 shadow_softness: Optional[float] = None):
         from .renderer import DeviceScene, default_renderer
         from .scenes import SceneArrays
 
@@ -895,6 +1170,10 @@ class DeviceMeshView:
                 raise ValueError("a textured view takes grey point lights [L, 4] only: its shade has one channel (or "
                                  "shading='phong_textured')")
         self.point_lights = point_lights
+        self.shadow_map_size = check_shadow_arguments(shading, point_lights, shadow_map_size, shadow_bias,
+                                                      shadow_softness)
+        self.shadow_bias = float(shadow_bias) if self.shadow_map_size else None
+        self.shadow_softness = float(shadow_softness) if self.shadow_map_size else None
         self._sh_scratch, self._sh_key = None, None
         if textured:
             if uv is None or faces_uv is None or texture is None:
@@ -965,6 +1244,49 @@ class DeviceMeshView:
             self._phong_scratch = new_scratch(self.device)
             self._phong_key = None
             self._phong_background = torch.from_numpy(background.astype(np.float32)).to(self.device)
+        if self.shadow_map_size:
+            self._cube = ShadowCubes(faces_u32, V, point_lights.shape[0], self.shadow_map_size, clockwise, self.device)
+
+    def _new_outputs(self, scene) -> dict:
+        return self.renderer._new_outputs(scene, False, False, False)
+
+    def shadow_maps(self) -> torch.Tensor:
+        """The cube shadow maps [6L, M, M] f32 of the last render (face 6 j + k: light j's +x, -x, +y, -y, +z, -z;
+        overwritten by the next render)."""
+        if not self.shadow_map_size:
+            raise ValueError("this view casts no shadows (shadow_map_size 0)")
+        return self._cube.maps
+
+    def shadow_visibility(self) -> torch.Tensor:
+        """The lights' visibility [H,W,L] f32 of the last render's pixels (1 where the coverage is 0)."""
+        if not self.shadow_map_size:
+            raise ValueError("this view casts no shadows (shadow_map_size 0)")
+        return self._saved[-1]
+
+    def _shade(self, gbuffer: torch.Tensor, params: torch.Tensor, center: torch.Tensor, background: torch.Tensor,
+               albedo: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """phong_shade of a G-buffer, under the lights' visibility in a view with shadows -> (image, vis or None)."""
+        vis = None
+        if self.shadow_map_size:
+            vis = shadow_visibility(gbuffer, self.point_lights, self._cube.maps, self.shadow_bias,
+                                    self.shadow_softness, albedo=albedo)
+        return phong_shade(gbuffer, params, center, background, sh=self.sh, albedo=albedo,
+                           point_lights=self.point_lights, visibility=vis), vis
+
+    def _shade_backward(self, gbuffer, params, center, background, image_b, camera_grad, albedo, vis):
+        """phong_shade_backward, and in a view with shadows the visibility's adjoint added into channels_b and lights_b
+        -> (the result of phong_shade_backward without vis_b, the cube maps' gradient [6L, M, M] or None)."""
+        shaded = phong_shade_backward(gbuffer, params, center, background, image_b, self._phong_scratch,
+                                      center_grad=camera_grad, sh=self.sh, albedo=albedo,
+                                      point_lights=self.point_lights, visibility=vis)
+        if vis is None:
+            return shaded, None
+        shaded, vis_b = shaded[:-1], shaded[-1]
+        _, maps_b, _ = shadow_visibility_backward(gbuffer, self.point_lights, self._cube.maps, self.shadow_bias,
+                                                  self.shadow_softness, vis_b, self._phong_scratch, albedo=albedo,
+                                                  channels_b=shaded[0], maps_b=self._cube.zero_maps_b(),
+                                                  lights_b=shaded[-1])
+        return shaded, maps_b
 
     def _phong_params(self) -> Tuple[torch.Tensor, torch.Tensor]:
         """(params [6], camera_center [3]) fp64 on the device, uploaded again only when the light, the specular
@@ -1089,30 +1411,44 @@ class DeviceMeshView:
         t["colors"][:, nc:nc + 3].copy_(normals)
         t["colors"][:, nc + 3:nc + 6].copy_(vertices)
         self.topology.edge_on_silhouette(ij, out=t["edgeflags"])
-        fwd = self.renderer.render(self._phong_scene, self.sigma)
+        if self.shadow_map_size:
+            # the G-buffer and the 6L cube faces in one call (one live forward per slot)
+            self._cube.prepare(vertices, self.point_lights)
+            fwds = self.renderer.render_views([self._phong_scene] + self._cube.scenes, self.sigma,
+                                              out=[self._new_outputs(self._phong_scene)] + self._cube.outputs())
+            fwd = fwds[0]
+            self._cube.fwds = fwds[1:]
+        else:
+            fwd = self.renderer.render(self._phong_scene, self.sigma)
         params, center = self._phong_params()
-        self._saved = (vertices, vertex_colors, normals, fwd, params, center)
-        return phong_shade(fwd["image"], params, center, self.scene.t["background_color"], sh=self.sh,
-                           point_lights=self.point_lights)
+        image, vis = self._shade(fwd["image"], params, center, self.scene.t["background_color"])
+        self._saved = (vertices, vertex_colors, normals, fwd, params, center, vis)
+        return image
 
     def _backward_phong(self, image_b: torch.Tensor, reference_transpose: bool,
                         camera_grad: bool) -> Dict[str, torch.Tensor]:
         # phong_shade_b -> channels_b; raster adjoint -> colors_b [V,K], ij_b; the albedo slice is vertex_colors_b, the
         # normal slice goes through the normal adjoint, the position slice adds to vertices_b, ij_b through the
         # projection's adjoint
-        vertices, _, _, fwd, params, center = self._saved
+        vertices, _, _, fwd, params, center, vis = self._saved
         nc = self.scene.nb_colors
-        shaded = phong_shade_backward(fwd["image"], params, center, self.scene.t["background_color"], image_b,
-                                      self._phong_scratch, center_grad=camera_grad, sh=self.sh,
-                                      point_lights=self.point_lights)
+        shaded, maps_b = self._shade_backward(fwd["image"], params, center, self.scene.t["background_color"], image_b,
+                                              camera_grad, None, vis)
         lights_b = None
         if self.point_lights is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
         channels_b, params_b = shaded[:2]
-        grads = self.renderer.render_b(self._phong_scene, self.sigma, fwd, channels_b)
+        if maps_b is not None:
+            grads = self.renderer.render_b_views([self._phong_scene] + self._cube.scenes, self.sigma,
+                                                 [fwd] + self._cube.fwds, [channels_b] + self._cube.image_bs(maps_b),
+                                                 [self._phong_scene.zero_grads()] + self._cube.grads())[0]
+        else:
+            grads = self.renderer.render_b(self._phong_scene, self.sigma, fwd, channels_b)
         colors_b = grads["colors_b"]
         vertices_b = self.topology.vertex_normals_backward(vertices, colors_b[:, nc:nc + 3])
         vertices_b += colors_b[:, nc + 3:nc + 6]
+        if maps_b is not None:
+            self._cube.backward(vertices, self.point_lights, vertices_b, lights_b, self._phong_scratch)
         _, camera_b = self._project_backward(vertices, grads["ij_b"], None, vertices_b, reference_transpose,
                                              camera_grad)
         out = {"vertices_b": vertices_b, "vertex_colors_b": colors_b[:, :nc].to(torch.float64),
@@ -1147,29 +1483,44 @@ class DeviceMeshView:
         g["colors"][:, 3:6].copy_(vertices)
         self.topology.edge_on_silhouette(ij, out=a["edgeflags"])
         g["edgeflags"].copy_(a["edgeflags"])
-        fwds = self.renderer.render_views([self.scene, self._phong_scene], self.sigma)
+        if self.shadow_map_size:
+            self._cube.prepare(vertices, self.point_lights)
+            fwds = self.renderer.render_views([self.scene, self._phong_scene] + self._cube.scenes, self.sigma,
+                                              out=[self._new_outputs(self.scene), self._new_outputs(self._phong_scene)]
+                                              + self._cube.outputs())
+            fwds, self._cube.fwds = fwds[:2], fwds[2:]
+        else:
+            fwds = self.renderer.render_views([self.scene, self._phong_scene], self.sigma)
         params, center = self._phong_params()
-        self._saved = (vertices, None, normals, fwds, params, center)
-        return phong_shade(fwds[1]["image"], params, center, self._phong_background, sh=self.sh,
-                           albedo=fwds[0]["image"], point_lights=self.point_lights)
+        image, vis = self._shade(fwds[1]["image"], params, center, self._phong_background, albedo=fwds[0]["image"])
+        self._saved = (vertices, None, normals, fwds, params, center, vis)
+        return image
 
     def _backward_phong_textured(self, image_b: torch.Tensor, reference_transpose: bool,
                                  camera_grad: bool) -> Dict[str, torch.Tensor]:
         # the shading's adjoint -> albedo_b, channels_b; one adjoint call over both rasters -> texture_b, uv_b and the
         # G-buffer's colors_b (normal slice through the normal adjoint, position slice into vertices_b); the two ij_b
         # are summed before the projection's adjoint.  The albedo raster's shade_b is not used: its shade is constant
-        vertices, _, _, fwds, params, center = self._saved
-        shaded = phong_shade_backward(fwds[1]["image"], params, center, self._phong_background, image_b,
-                                      self._phong_scratch, center_grad=camera_grad, sh=self.sh, albedo=fwds[0]["image"],
-                                      point_lights=self.point_lights)
+        vertices, _, _, fwds, params, center, vis = self._saved
+        shaded, maps_b = self._shade_backward(fwds[1]["image"], params, center, self._phong_background, image_b,
+                                              camera_grad, fwds[0]["image"], vis)
         lights_b = None
         if self.point_lights is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
         channels_b, params_b, albedo_b = shaded[0], shaded[1], shaded[-1]
-        ga, gg = self.renderer.render_b_views([self.scene, self._phong_scene], self.sigma, fwds, [albedo_b, channels_b])
+        if maps_b is not None:
+            ga, gg = self.renderer.render_b_views(
+                [self.scene, self._phong_scene] + self._cube.scenes, self.sigma, list(fwds) + self._cube.fwds,
+                [albedo_b, channels_b] + self._cube.image_bs(maps_b),
+                [self.scene.zero_grads(), self._phong_scene.zero_grads()] + self._cube.grads())[:2]
+        else:
+            ga, gg = self.renderer.render_b_views([self.scene, self._phong_scene], self.sigma, fwds,
+                                                  [albedo_b, channels_b])
         colors_b = gg["colors_b"]
         vertices_b = self.topology.vertex_normals_backward(vertices, colors_b[:, 0:3])
         vertices_b += colors_b[:, 3:6]
+        if maps_b is not None:
+            self._cube.backward(vertices, self.point_lights, vertices_b, lights_b, self._phong_scratch)
         _, camera_b = self._project_backward(vertices, ga["ij_b"] + gg["ij_b"], None, vertices_b,
                                              reference_transpose, camera_grad)
         out = {"vertices_b": vertices_b, "texture_b": ga["texture_b"], "uv_b": ga["uv_b"], "light_b": params_b[:4],

@@ -33,6 +33,12 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
     RenderMeshPhongTexturedFunc  (ij, uv, texture, channels [V,7], depths, edgeflags, albedo scene, G-buffer scene,
                            sigma) -> (albedo [H,W,C], G-buffer [H,W,7]): the two rasters of a textured Phong render
                            in one forward call and one adjoint call; gradients to ij, uv, texture and channels
+    RenderShadowedPhongFunc  (ij, uv | None, texture | None, channels, depths, edgeflags, vertices, point_lights,
+                           albedo scene | None, G-buffer scene, ShadowCubes, sigma) -> ([albedo,] G-buffer, cube maps
+                           [6L,M,M]): a Phong render's raster(s) and the lights' cube shadow maps in one forward call
+                           and one adjoint call; the maps' share reaches the vertices and the lights' positions
+    ShadowVisibilityFunc   (G-buffer, point_lights, maps, bias, softness, albedo | None) -> visibility [H,W,L]; the
+                           G-buffer, the maps and the lights' positions receive their gradients
 
 All maths is fp64 but the rasteriser's (fp32 image and image gradients).  ``RenderMesh2DFunc``,
 ``RenderMesh2DTexturedFunc`` and ``RenderMeshPhongTexturedFunc`` follow the snapshot / replay rule of the 2D Functions (differentiable_renderer_pytorch.py):
@@ -49,7 +55,9 @@ import torch
 
 from ..mesh_fitter import DeviceLaplacianRigidEnergy, new_scratch, pose, pose_backward
 from ..mesh_ops import (CameraParams, LoopSubdivision, MeshTopology, camera_center, lit_vertex_colors,
-                        lit_vertex_colors_backward, phong_shade, phong_shade_backward, project_points,
+                        ShadowCubes, check_shadow_arguments, cube_project_backward, lit_vertex_colors_backward,
+                        phong_shade, phong_shade_backward, project_points, shadow_visibility,
+                        shadow_visibility_backward,
                         point_lit_vertex_colors, point_lit_vertex_colors_backward, sh_lit_vertex_colors,
                         sh_lit_vertex_colors_backward,
                         project_points_backward_f64, project_points_camera_backward, project_points_dev)
@@ -440,7 +448,7 @@ class PhongShadeFunc(torch.autograd.Function):
     def forward(ctx: Any, channels: torch.Tensor, light_directional: Optional[torch.Tensor],  # type: ignore
                 light_ambient, specular, shininess, camera: CameraParams, background,
                 sh: Optional[torch.Tensor] = None, albedo: Optional[torch.Tensor] = None,
-                point_lights: Optional[torch.Tensor] = None):
+                point_lights: Optional[torch.Tensor] = None, visibility: Optional[torch.Tensor] = None):
         dev = channels.device
         scalars = [x if isinstance(x, torch.Tensor) else torch.tensor(float(x), dtype=torch.float64, device=dev)
                    for x in (light_ambient, specular, shininess)]
@@ -459,8 +467,10 @@ class PhongShadeFunc(torch.autograd.Function):
         shd = _f64(sh) if sh is not None else None
         alb = albedo.detach().to(torch.float32).contiguous() if albedo is not None else None
         pl = _f64(point_lights) if point_lights is not None else None
-        image = phong_shade(ch, params, center, bg, sh=shd, albedo=alb, point_lights=pl)
-        ctx.save_for_backward(ch, params, center, bg.to(dev, torch.float32), shd, alb, pl)
+        vis = visibility.detach().to(torch.float32).contiguous() if visibility is not None else None
+        image = phong_shade(ch, params, center, bg, sh=shd, albedo=alb, point_lights=pl, visibility=vis)
+        ctx.save_for_backward(ch, params, center, bg.to(dev, torch.float32), shd, alb, pl, vis)
+        ctx.vis_dtype = visibility.dtype if visibility is not None else None
         ctx.lights_dtype = point_lights.dtype if point_lights is not None else None
         ctx.albedo_dtype = albedo.dtype if albedo is not None else None
         ctx.sh_dtype = sh.dtype if sh is not None else None
@@ -471,11 +481,14 @@ class PhongShadeFunc(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx: Any, image_b: torch.Tensor):  # type: ignore
-        ch, params, center, bg, shd, alb, pl = ctx.saved_tensors
+        ch, params, center, bg, shd, alb, pl, vis = ctx.saved_tensors
         needs = ctx.needs_input_grad
         center_grad = ctx.center_is_input and needs[5]
         shaded = phong_shade_backward(ch, params, center, bg, image_b, _scratch_of(ch.device), center_grad=center_grad,
-                                      sh=shd, albedo=alb, point_lights=pl)
+                                      sh=shd, albedo=alb, point_lights=pl, visibility=vis)
+        vis_b = None
+        if vis is not None:
+            shaded, vis_b = shaded[:-1], shaded[-1]
         lights_b = None
         if pl is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
@@ -493,7 +506,121 @@ class PhongShadeFunc(torch.autograd.Function):
         out.append(shaded[-1].to(ctx.sh_dtype) if shd is not None and needs[7] else None)
         out.append(albedo_b.to(ctx.albedo_dtype) if albedo_b is not None and needs[8] else None)
         out.append(lights_b.to(ctx.lights_dtype) if lights_b is not None and needs[9] else None)
+        out.append(vis_b.to(ctx.vis_dtype) if vis_b is not None and needs[10] else None)
         return tuple(out)
+
+
+class RenderShadowedPhongFunc(torch.autograd.Function):
+    """The rasters of a Phong render with shadows, as one node: the G-buffer (beside the albedo raster of a textured
+    mesh, as ``RenderMeshPhongTexturedFunc``) and the 6L cube shadow maps of the point lights (``ShadowCubes``, the
+    model in include/deodr_b200.h), rendered by one ``render_views`` call and back-propagated by one
+    ``render_b_views`` call, the renderer keeping one live forward per slot.  (ij, uv | None, texture | None, channels,
+    depths, edgeflags, vertices [V,3], point_lights [L, 3 + S], albedo scene | None, G-buffer scene, cubes, sigma) ->
+    ([albedo [H,W,C],] G-buffer, maps [6L,M,M]) fp32.  The cube projection happens inside the node, so the maps'
+    gradient reaches the vertices and the lights' positions through its adjoint.  Same snapshot / replay rule as
+    ``RenderMesh2DFunc``."""
+
+    NAMES = ("ij", "uv", "shade", "texture")
+
+    @staticmethod
+    def forward(ctx: Any, ij: torch.Tensor, uv: Optional[torch.Tensor], texture: Optional[torch.Tensor],  # type: ignore
+                channels: torch.Tensor, depths: torch.Tensor, edgeflags: torch.Tensor, vertices: torch.Tensor,
+                point_lights: torch.Tensor, albedo_scene: Optional[DeviceScene], gbuffer_scene: DeviceScene,
+                cubes: ShadowCubes, sigma: float = 1.0):
+        textured = albedo_scene is not None
+        if textured:
+            check_scene_inputs(albedo_scene, uv=uv, texture=texture)
+        check_scene_inputs(gbuffer_scene, colors=channels)
+        inputs = (ij.detach(), uv.detach() if textured else None, texture.detach() if textured else None,
+                  channels.detach(), depths.detach(), edgeflags, _f64(vertices.detach()), _f64(point_lights.detach()))
+        ctx.scenes = ([albedo_scene] if textured else []) + [gbuffer_scene]
+        ctx.cubes, ctx.sigma, ctx.textured = cubes, float(sigma), textured
+        renderer = default_renderer(gbuffer_scene.device.index)
+        ctx.fwds = RenderShadowedPhongFunc._render(renderer, ctx, inputs, None)
+        ctx.in_dtypes = (ij.dtype, uv.dtype if textured else None, texture.dtype if textured else None, channels.dtype,
+                         vertices.dtype, point_lights.dtype)
+        ctx.save_for_backward(*(t.clone() if t is not None else None for t in inputs))
+        rasters = tuple(f["image"].clone() for f in ctx.fwds[:len(ctx.scenes)])
+        return rasters + (cubes.maps.clone(),)
+
+    @staticmethod
+    def _render(renderer, ctx, inputs, out):
+        ij, uv, texture, channels, depths, edgeflags, vertices, lights = inputs
+        if ctx.textured:
+            ctx.scenes[0].update(ij=ij, uv=uv, texture=texture, depths=depths, edgeflags=edgeflags)
+        ctx.scenes[-1].update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
+        ctx.cubes.prepare(vertices, lights)
+        if out is None:
+            out = [renderer._new_outputs(sc, False, False, False) for sc in ctx.scenes] + ctx.cubes.outputs()
+        return renderer.render_views(ctx.scenes + ctx.cubes.scenes, ctx.sigma, out=out)
+
+    @staticmethod
+    def backward(ctx: Any, *grads):  # type: ignore
+        needs = ctx.needs_input_grad
+        if not any(needs[:8]):
+            return (None,) * 12
+        inputs = ctx.saved_tensors
+        renderer = default_renderer(ctx.scenes[-1].device.index)
+        n = len(ctx.scenes)
+        # the shared scenes and cubes may hold another node's inputs by now
+        if any(f["generation"] != renderer.generation(f["slot"]) for f in ctx.fwds):
+            ctx.fwds = RenderShadowedPhongFunc._render(renderer, ctx, inputs, ctx.fwds)
+        else:
+            if ctx.textured:
+                ctx.scenes[0].update(ij=inputs[0], uv=inputs[1], texture=inputs[2], depths=inputs[4],
+                                     edgeflags=inputs[5])
+            ctx.scenes[-1].update(ij=inputs[0], colors=inputs[3], depths=inputs[4], edgeflags=inputs[5])
+            ctx.cubes.prepare(inputs[6], inputs[7])
+        if ctx.textured:
+            gs = [requested_grads(ctx.scenes[0], RenderShadowedPhongFunc.NAMES, (True, needs[1], False, needs[2])),
+                  ctx.scenes[1].zero_grads()]
+        else:
+            gs = [ctx.scenes[0].zero_grads()]
+        image_bs = [g.to(torch.float32).contiguous() for g in grads[:n]]
+        maps_b = grads[n].to(torch.float32).contiguous()
+        renderer.render_b_views(ctx.scenes + ctx.cubes.scenes, ctx.sigma, ctx.fwds,
+                                image_bs + ctx.cubes.image_bs(maps_b), grads=gs + ctx.cubes.grads())
+        vertices_b, lights_b = cube_project_backward(inputs[6], inputs[7], ctx.cubes.M, ctx.cubes.cameras,
+                                                     ctx.cubes.ij_b, ctx.cubes.colors_b.view(6 * ctx.cubes.L, -1),
+                                                     _scratch_of(inputs[6].device))
+        ij_d, uv_d, tex_d, ch_d, v_d, l_d = ctx.in_dtypes
+        ij_b = sum(g["ij_b"] for g in gs)
+        return (ij_b.to(ij_d) if needs[0] else None,
+                gs[0]["uv_b"].to(uv_d) if ctx.textured and needs[1] else None,
+                gs[0]["texture_b"].to(tex_d) if ctx.textured and needs[2] else None,
+                gs[-1]["colors_b"].to(ch_d) if needs[3] else None, None, None,
+                vertices_b.to(v_d) if needs[6] else None, lights_b.to(l_d) if needs[7] else None,
+                None, None, None, None)
+
+
+class ShadowVisibilityFunc(torch.autograd.Function):
+    """The point lights' visibility of a G-buffer's pixels (deodr_b200_shadow_visibility / _b, the model in
+    include/deodr_b200.h): (channels [H,W,C+7], or [H,W,7] beside an albedo, point_lights [L, 3 + S], maps [6L,M,M],
+    bias, softness, albedo | None) -> visibility [H,W,L] fp32.  Backward returns the gradients of the G-buffer's
+    position and coverage slices, of the maps and of the lights' positions; the albedo, only read for its channel
+    count, gets none."""
+
+    @staticmethod
+    def forward(ctx: Any, channels: torch.Tensor, point_lights: torch.Tensor, maps: torch.Tensor,  # type: ignore
+                bias: float, softness: float, albedo: Optional[torch.Tensor] = None):
+        ch = channels.detach().to(torch.float32).contiguous()
+        pl, mp = _f64(point_lights.detach()), maps.detach().to(torch.float32).contiguous()
+        alb = albedo.detach() if albedo is not None else None
+        vis = shadow_visibility(ch, pl, mp, bias, softness, albedo=alb)
+        ctx.save_for_backward(ch, pl, mp, alb)
+        ctx.band = (float(bias), float(softness))
+        ctx.dtypes = (channels.dtype, point_lights.dtype, maps.dtype)
+        return vis
+
+    @staticmethod
+    def backward(ctx: Any, vis_b: torch.Tensor):  # type: ignore
+        ch, pl, mp, alb = ctx.saved_tensors
+        channels_b, maps_b, lights_b = shadow_visibility_backward(ch, pl, mp, *ctx.band, vis_b, _scratch_of(ch.device),
+                                                                  albedo=alb)
+        needs = ctx.needs_input_grad
+        cd, ld, md = ctx.dtypes
+        return (channels_b.to(cd) if needs[0] else None, lights_b.to(ld) if needs[1] else None,
+                maps_b.to(md) if needs[2] else None, None, None, None)
 
 
 project_points_autograd = ProjectPointsFunc.apply
@@ -508,6 +635,8 @@ pose_autograd = PoseFunc.apply
 rigid_energy_autograd = RigidEnergyFunc.apply
 loop_subdivision_autograd = LoopSubdivisionFunc.apply
 phong_shade_autograd = PhongShadeFunc.apply
+render_shadowed_phong = RenderShadowedPhongFunc.apply
+shadow_visibility_autograd = ShadowVisibilityFunc.apply
 
 
 def vertex_luminosity_autograd(normals: torch.Tensor, light_directional: Optional[torch.Tensor],
@@ -684,7 +813,10 @@ class Scene3DPytorch:
 
     ``set_point_lights`` adds point lights near the mesh in every shading; a table that requires grad receives its
     gradient, and the vertices receive the lights' share through their normals and their positions.  A flash is a
-    light whose position the caller computes from the camera's tensors: its gradient then reaches the camera."""
+    light whose position the caller computes from the camera's tensors: its gradient then reaches the camera.  In a
+    Phong or textured Phong render, ``set_point_lights(..., shadow_map_size=M)`` makes them cast shadows (the model in
+    include/deodr_b200.h): the rasters and the lights' cube maps are one :class:`RenderShadowedPhongFunc` node, the
+    visibility a :class:`ShadowVisibilityFunc`, and the shadows' gradient reaches the vertices and the lights."""
 
     def __init__(self, sigma: float = 1.0, backface_culling: bool = True, shading: str = "gouraud"):
         if shading not in ("gouraud", "phong", "phong_textured"):
@@ -697,6 +829,8 @@ class Scene3DPytorch:
         self.light_ambient: Optional[torch.Tensor] = None
         self.light_sh: Optional[torch.Tensor] = None
         self.point_lights: Optional[torch.Tensor] = None
+        self.shadow_map_size, self.shadow_bias, self.shadow_softness = 0, None, None
+        self._cubes: Dict[tuple, ShadowCubes] = {}
         self.specular: Any = 0.0
         self.shininess: Any = 16.0
         self.background_color: Optional[np.ndarray] = None
@@ -706,6 +840,7 @@ class Scene3DPytorch:
 
     def set_mesh(self, mesh: ColoredTriMeshPytorch) -> None:
         self.mesh = mesh
+        self._cubes = {}
         self._scenes = {}
         self._phong_scenes = {}
         self._albedo_scenes = {}
@@ -741,11 +876,18 @@ class Scene3DPytorch:
                 raise ValueError(f"sh must be [9] or [9,C] with C from 1 to 4; got {tuple(sh.shape)}")
         self.light_sh = sh
 
-    def set_point_lights(self, lights) -> None:
+    def set_point_lights(self, lights, shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
+                         shadow_softness: Optional[float] = None) -> None:
         """Point lights added to the light (the model in include/deodr_b200.h): [L, 3 + S], row j the light's world
         position then its intensity, grey (S = 1) or one per channel (S = C up to 4), L from 1 to 8; a tensor used as
         given (so one that requires grad, or one computed from other tensors, receives its gradient) or an array.
-        None removes them.  A textured mesh takes grey lights only, unless it is shaded per pixel."""
+        None removes them.  A textured mesh takes grey lights only, unless it is shaded per pixel.  A
+        ``shadow_map_size`` M > 0 makes them cast shadows in a Phong render, with ``shadow_bias`` and
+        ``shadow_softness`` (world units, both required) and the refusals of ``DeviceMeshView``."""
+        size = check_shadow_arguments(self.shading, lights, shadow_map_size, shadow_bias, shadow_softness)
+        self.shadow_map_size = size
+        self.shadow_bias = float(shadow_bias) if size else None
+        self.shadow_softness = float(shadow_softness) if size else None
         if lights is not None:
             dev = self.mesh.device if self.mesh is not None else _device(None)
             if not isinstance(lights, torch.Tensor):
@@ -840,12 +982,21 @@ class Scene3DPytorch:
         ij, depths = camera.project_points(m.vertices)
         ones = torch.ones((m.nb_vertices, 1), dtype=torch.float64, device=m.device)
         channels = torch.cat((m.vertex_normals, m.vertices.to(torch.float64), ones), dim=1)
-        albedo, gbuffer = render_mesh_phong_textured(ij, uv, texture, channels, depths, self._edgeflags(ij),
-                                                     self._albedo_scene(camera, uv, texture),
-                                                     self._phong_scene(camera, 0), self.sigma)
+        vis = None
+        if self.shadow_map_size:
+            albedo, gbuffer, maps = render_shadowed_phong(ij, uv, texture, channels, depths, self._edgeflags(ij),
+                                                          m.vertices, self.point_lights,
+                                                          self._albedo_scene(camera, uv, texture),
+                                                          self._phong_scene(camera, 0), self._shadow_cubes(), self.sigma)
+            vis = shadow_visibility_autograd(gbuffer, self.point_lights, maps, self.shadow_bias, self.shadow_softness,
+                                             albedo)
+        else:
+            albedo, gbuffer = render_mesh_phong_textured(ij, uv, texture, channels, depths, self._edgeflags(ij),
+                                                         self._albedo_scene(camera, uv, texture),
+                                                         self._phong_scene(camera, 0), self.sigma)
         return phong_shade_autograd(gbuffer, self.light_directional, self.light_ambient, self.specular,
                                     self.shininess, camera.center() if camera.is_tensor else camera,
-                                    self.background_color, self.light_sh, albedo, self.point_lights)
+                                    self.background_color, self.light_sh, albedo, self.point_lights, vis)
 
     def _render_phong(self, camera: CameraPytorch) -> torch.Tensor:
         m = self.mesh
@@ -861,10 +1012,27 @@ class Scene3DPytorch:
         ones = torch.ones((m.nb_vertices, 1), dtype=torch.float64, device=m.device)
         channels = torch.cat((m.vertices_colors.to(torch.float64), m.vertex_normals, m.vertices.to(torch.float64),
                               ones), dim=1)
-        raster = render_mesh_2d(ij, channels, depths, self._edgeflags(ij), self._phong_scene(camera, nc), self.sigma)
+        vis = None
+        if self.shadow_map_size:
+            raster, maps = render_shadowed_phong(ij, None, None, channels, depths, self._edgeflags(ij), m.vertices,
+                                                 self.point_lights, None, self._phong_scene(camera, nc),
+                                                 self._shadow_cubes(), self.sigma)
+            vis = shadow_visibility_autograd(raster, self.point_lights, maps, self.shadow_bias, self.shadow_softness)
+        else:
+            raster = render_mesh_2d(ij, channels, depths, self._edgeflags(ij), self._phong_scene(camera, nc),
+                                    self.sigma)
         return phong_shade_autograd(raster, self.light_directional, self.light_ambient, self.specular, self.shininess,
                                     camera.center() if camera.is_tensor else camera, self.background_color,
-                                    self.light_sh, None, self.point_lights)
+                                    self.light_sh, None, self.point_lights, vis)
+
+    def _shadow_cubes(self) -> ShadowCubes:
+        """The cached cube shadow maps of the mesh for the lights' count and the map size."""
+        m = self.mesh
+        key = (self.point_lights.shape[0], self.shadow_map_size)
+        if key not in self._cubes:
+            self._cubes[key] = ShadowCubes(np.ascontiguousarray(m.faces, dtype=np.uint32), m.nb_vertices, key[0],
+                                           key[1], m.clockwise, m.device)
+        return self._cubes[key]
 
     def _edgeflags(self, ij: torch.Tensor) -> torch.Tensor:
         if self.sigma > 0:

@@ -611,7 +611,8 @@ int deodr_b200_phong_shade_albedo_b(const DeodrPhongIO *io, const float *albedo,
  * with x_v the vertex's world position, no specular term per vertex, and per pixel x = X / a, v, a, ks and e those of
  * DeodrPhongIO; every point-light term is 0 where a = 0.  Without an environment its term is left out.  The
  * max(0, .) gates read `> 0`, so a NaN normal gives a zero point-light term, and a table of zero intensities gives bit
- * for bit the outputs of the calls without point lights.  No visibility or shadowing.
+ * for bit the outputs of the calls without point lights.  No visibility here: per pixel, shadows are the
+ * shadowed calls below.
  *
  * Adjoint: lights_b [L, 3 + S] is the gradient of every entry, summed in fp64 in a fixed order without atomics
  * (bit-reproducible; `scratch` as above).  The normals receive sum_j of the terms' normal gradients (Phong: through
@@ -652,6 +653,88 @@ int deodr_b200_point_phong_shade(const DeodrPhongIO *io, const float *albedo, co
 int deodr_b200_point_phong_shade_b(const DeodrPhongIO *io, const float *albedo, float *albedo_b, const double *sh,
                                    int sh_channels, double *sh_b, const double *lights, int nb_lights,
                                    int light_channels, double *lights_b, double *scratch, void *stream);
+
+/* ---- shadows from point lights --------------------------------------------------------------------------------------
+ * Every light j of a point-light table lights [L, 3 + S] gets a cube shadow map: six depth renders of the mesh, each
+ * M x M (M from 8 to 4096), seen from p_j.  Face f = 6 j + k (k = 0..5: +x, -x, +y, -y, +z, -z) is the camera vector
+ * [26] of the device-camera entry points with
+ *
+ *   extrinsic [R_k | -R_k p_j],  intrinsic [[phi, 0, (M-1)/2], [0, phi, (M-1)/2], [0, 0, 1]],  phi = M/2 - 2,
+ *   no distortion, and the rows of R_k (the camera's x, y and z axes in world coordinates; each a proper rotation,
+ *   so that every face keeps the mesh's winding):
+ *     +x: (0,1,0) (0,0,1) (1,0,0)     -x: (0,0,1) (0,1,0) (-1,0,0)
+ *     +y: (0,0,1) (1,0,0) (0,1,0)     -y: (1,0,0) (0,0,1) (0,-1,0)
+ *     +z: (1,0,0) (0,1,0) (0,0,1)     -z: (0,1,0) (1,0,0) (0,0,-1)
+ *
+ * A face is slightly wider than 90 degrees, so that the 2x2 taps of a point on a face boundary stay inside its map.
+ * The map D_f [M,M] (row v, column u) is the depth render of the mesh through that camera: the vertex depth as a
+ * one-channel colour, antialiased with the caller's sigma in map pixels, with the mesh's winding and backface culling
+ * on, over a background depth DEODR_B200_SHADOW_FAR (finite, so that the silhouette blend beta z + (1 - beta) FAR
+ * stays finite).  The visibility of a surface point x (per pixel x = X / a, as for the point-light terms):
+ *
+ *   d = x - p_j;  k = the dominant axis of d with its sign (ties go to x, then y, then z);  f = 6 j + k
+ *   (u, v, z) = the projection of x through face f (the arithmetic of deodr_b200_project_points_dev)
+ *   taps: the 2x2 neighbourhood (u0, v0) = floor(u, v), (fu, fv) = (u - u0, v - v0), indices clamped into [0, M)
+ *   s_k = s((D_f[tap k] + bias - z) / softness + 1),  s(y) = 3 y^2 - 2 y^3 on y clamped to [0, 1]
+ *   V_j = lerp(lerp(s_00, s_10, fu), lerp(s_01, s_11, fu), fv),  lerp(a, b, t) = a + t (b - a)
+ *
+ * s is exactly 1 when D + bias >= z and exactly 0 when D + bias <= z - softness, and the lerps give V = 1 exactly when
+ * every tap is 1.  bias > 0 and softness > 0 are world units.  V_j = 1 where a = 0, and where the projection is not in
+ * front of the face or not finite (x at the light, or a NaN position).  Shading: per pixel, light j's diff_j and
+ * spec_j (the point-light terms above) are multiplied by V_j, each product rounded on its own, so that where every V_j
+ * is 1 the image is bit for bit the image of deodr_b200_point_phong_shade.  Every other term is unchanged.
+ *
+ * Adjoint: from vis_b [H,W,L], the gradient goes to x (through z and the bilinear weights; into the G-buffer's
+ * position slice and, through x = X / a, its coverage slice), to the map texels (fp32 atomics) and to p_j through
+ * t_f = -R_f p_j (the face choice is piecewise constant).  The maps' gradient then goes through the rasteriser's
+ * adjoint of the 6L face renders, whose depths_b (= colors_b) and ij_b the cube projection's adjoint takes to the
+ * vertices and to p_j.
+ *
+ * Limitations: a triangle with a vertex behind a face's camera plane is missing from that face's map (the rasteriser
+ * drops it with culling on), which happens only for a triangle that subtends more than 45 degrees at the light; open
+ * surfaces cast shadows from their front side only; at the view's self-occlusion silhouettes x is the G-buffer's
+ * mixed position (the Phong approximation); D and the G-buffer's X are both interpolated linearly in screen space, so
+ * a lit surface's own z and D differ by an amount that grows with triangle size, which bias must cover. */
+#define DEODR_B200_SHADOW_FAR 1e30
+
+/* The cube cameras and the projection of vertices [n,3] through them: cameras [6L, 26] (face f = 6 j + k), ij
+ * [6L, n, 2] and depths [6L, n] fp64, all written; face f's are bit-identical to deodr_b200_project_points_dev with
+ * camera vector cameras[f] and no distortion.  The lights stay in device memory (nothing is read back).
+ * DEODR_B200_EINVAL for n < 1, a NULL buffer or map_size outside [8, 4096]; DEODR_B200_EUNSUPPORTED for nb_lights
+ * outside [1, 8] or light_channels outside [1, 4]; both before any launch.  No host synchronisation. */
+int deodr_b200_cube_project(const double *vertices, int n, const double *lights, int nb_lights, int light_channels,
+                            int map_size, double *cameras, double *ij, double *depths, void *stream);
+/* Its adjoint from ij_b [6L, n, 2] and depths_b [6L, n] (fp32, the rasteriser's): vertices_b [n,3] accumulated, one
+ * thread per vertex adding its 6L faces in order (no atomics), and the position entries lights_b[j, 0:3] accumulated
+ * with the faces' share -sum_k R_k^T t_b, summed in a fixed order (`scratch` of deodr_b200_fitter_scratch_bytes).
+ * Same refusals, plus a NULL cameras (those of the forward), vertices_b, lights_b or scratch. */
+int deodr_b200_cube_project_b(const double *vertices, int n, const double *lights, int nb_lights, int light_channels,
+                              int map_size, const double *cameras, const float *ij_b, const float *depths_b,
+                              double *vertices_b, double *lights_b, double *scratch, void *stream);
+/* The visibility vis [H,W,L] fp32 of the G-buffer's pixels (io's channels, H, W, C, off_position and off_coverage,
+ * with a stride of C + 7, or 7 with off_albedo -1; nothing else of io is read) under the lights' cube maps maps
+ * [6L, M, M] fp32.  DEODR_B200_EINVAL for a NULL buffer, bad io sizes or offsets, map_size outside [8, 4096], or a
+ * non-finite or non-positive bias or softness; DEODR_B200_EUNSUPPORTED for nb_lights or light_channels outside the
+ * point-light rules; both before any launch.  No host synchronisation. */
+int deodr_b200_shadow_visibility(const DeodrPhongIO *io, const double *lights, int nb_lights, int light_channels,
+                                 const float *maps, int map_size, double bias, double softness, float *vis,
+                                 void *stream);
+/* Its adjoint from vis_b [H,W,L] fp32: io->channels_b's position and coverage slices accumulated, maps_b [6L,M,M]
+ * accumulated with fp32 atomics, and lights_b[j, 0:3] accumulated, summed in a fixed order.  Same refusals, plus a
+ * NULL channels_b, vis_b, maps_b, lights_b or scratch. */
+int deodr_b200_shadow_visibility_b(const DeodrPhongIO *io, const double *lights, int nb_lights, int light_channels,
+                                   const float *maps, int map_size, double bias, double softness, const float *vis_b,
+                                   float *maps_b, double *lights_b, double *scratch, void *stream);
+/* deodr_b200_point_phong_shade with light j's terms multiplied by vis [H,W,L] fp32 (its refusals, plus a NULL vis). */
+int deodr_b200_point_phong_shade_shadowed(const DeodrPhongIO *io, const float *albedo, const double *sh,
+                                          int sh_channels, const double *lights, int nb_lights, int light_channels,
+                                          const float *vis, void *stream);
+/* deodr_b200_point_phong_shade_b of the shadowed shading, which also writes vis_b [H,W,L] fp32 =
+ * sum_c image_b[c] (A[c] I_j[c] diff_j + I_j[c] spec_j) (0 where a = 0).  Its refusals, plus a NULL vis or vis_b. */
+int deodr_b200_point_phong_shade_shadowed_b(const DeodrPhongIO *io, const float *albedo, float *albedo_b,
+                                            const double *sh, int sh_channels, double *sh_b, const double *lights,
+                                            int nb_lights, int light_channels, double *lights_b, const float *vis,
+                                            float *vis_b, double *scratch, void *stream);
 
 /* One parameter vector of a heavy-ball update (device pointers, `size` entries each):
  *   step = clamp(-grad * factor, -max_step, max_step)   (max_step = INFINITY: unclamped)
