@@ -361,6 +361,24 @@ SYMBOLS = [
     ("deodr_b200_point_phong_shade_shadowed_b", C.c_int,
      [C.POINTER(PhongIO), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_sun_project", C.c_int,
+     [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_double), C.c_double, C.c_int, C.c_void_p, C.c_void_p,
+      C.c_void_p]),
+    ("deodr_b200_sun_project_b", C.c_int,
+     [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_double), C.c_double, C.c_int, C.c_void_p, C.c_void_p,
+      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_sun_visibility", C.c_int,
+     [C.POINTER(PhongIO), C.POINTER(C.c_double), C.c_double, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p,
+      C.c_void_p]),
+    ("deodr_b200_sun_visibility_b", C.c_int,
+     [C.POINTER(PhongIO), C.POINTER(C.c_double), C.c_double, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p,
+      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_phong_shade_sun_shadowed", C.c_int,
+     [C.POINTER(PhongIO), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+      C.c_void_p]),
+    ("deodr_b200_phong_shade_sun_shadowed_b", C.c_int,
+     [C.POINTER(PhongIO), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("deodr_b200_fitter_update", C.c_int,
      [C.POINTER(HeavyBall), C.c_void_p, C.POINTER(HeavyBall), C.c_int, C.c_double, C.c_double, C.c_void_p,
       C.c_void_p, C.c_void_p, C.c_void_p]),

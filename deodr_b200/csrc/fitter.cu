@@ -902,17 +902,25 @@ __device__ __forceinline__ float &albedo_b_at(float *pb, const DeodrPhongIO &io,
 // the registers of one CTA per SM (ptxas -v, DESIGN.md section 12).  With P > 0, point lights [L, 3 + P] add P_c to
 // the luminosity and Q_c to the specular term (P = 1: grey); at P = 3 the default budget spills 12 bytes across the
 // pow calls, so the point-light instances take one CTA's registers too (DESIGN.md section 13).  With VIS (P > 0), light
-// j's diffuse and specular terms are multiplied by its visibility vis [H,W,L] (DESIGN.md section 14)
-template <int S, bool SPLIT, int P = 0, bool VIS = false>
+// j's diffuse and specular terms are multiplied by its visibility vis [H,W,L] (DESIGN.md section 14); with SUN, the
+// directional light's by sun_vis [H,W] (DESIGN.md section 15)
+template <int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false>
 __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(DeodrPhongIO io, const double *sh,
                                                                   const float *albedo, const double *lights, int L,
-                                                                  const float *vis = nullptr) {
+                                                                  const float *vis = nullptr,
+                                                                  const float *sun_vis = nullptr) {
     const long long p = (long long)blockIdx.x * NT + threadIdx.x;
     if (p >= (long long)io.H * io.W) return;
     const int C = io.C;
     const float *px = io.channels + p * gbuffer_stride<SPLIT>(C);
     PhongTerms t;
     phong_terms(px, io, io.params, io.camera_center, t);
+    if constexpr (SUN) {
+        // each product rounded on its own, so that V = 1 leaves the terms, and the image, bit for bit
+        const double sv = sun_vis[p];
+        t.lum = io.params[3] + __dmul_rn(directional_of(t.dot_nl), sv);
+        t.spec = __dmul_rn(t.spec, sv);
+    }
     float *out = io.image + p * C;
     if constexpr (P > 0) {
         // pd[c] = P_c and qs[c] = Q_c, the lights in index order; both 0 where a = 0
@@ -986,13 +994,14 @@ __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(Deod
 // With point lights (P > 0) the albedo, normal, position and coverage adjoints, params_b and camera_center_b take their
 // share; lights_b is summed by k_point_lights_pixel_b, a pass of its own (up to 8 (3 + P) sums).
 // With VIS, light j's terms are scaled by vis [H,W,L] and vis_b[p, j] = alpha_j diff_j + beta_j spec_j is written
-// (0 where a = 0).
-template <bool CENTER, int S, bool SPLIT, int P = 0, bool VIS = false>
-__global__ void __launch_bounds__(NT, S == 2 || S == 4 ? 1 : 0) k_phong_shade_b(DeodrPhongIO io, Scratch *s,
-                                                                            const double *sh, const float *albedo,
-                                                                            float *albedo_b, const double *lights,
-                                                                            int L, const float *vis = nullptr,
-                                                                            float *vis_b = nullptr) {
+// (0 where a = 0).  With SUN, the directional diff and spec are scaled by sun_vis [H,W] and sun_vis_b[p] =
+// sum_c g_c (A_c diff + spec) is written; at S = 3 without point lights the default budget spills then too, so
+// those take one CTA's registers (DESIGN.md section 15).
+template <bool CENTER, int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false>
+__global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P == 0) ? 1 : 0)
+    k_phong_shade_b(DeodrPhongIO io, Scratch *s, const double *sh, const float *albedo, float *albedo_b,
+                    const double *lights, int L, const float *vis = nullptr, float *vis_b = nullptr,
+                    const float *sun_vis = nullptr, float *sun_vis_b = nullptr) {
     constexpr int NC = S > P ? S : P;
     constexpr int K = PHONG_SUMS + (CENTER ? 3 : 0);
     __shared__ double tot[K];
@@ -1108,6 +1117,13 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 ? 1 : 0) k_phong_shade_b(
         }
         PhongTerms t;
         phong_terms(px, io, prm, io.camera_center, t);
+        double sv = 1.0, diff0 = 0, spec0 = 0;  // with SUN: V and the unshadowed directional terms
+        if constexpr (SUN) {
+            sv = sun_vis[p];
+            diff0 = directional_of(t.dot_nl);
+            spec0 = t.spec;
+            t.lum = prm[3] + __dmul_rn(diff0, sv);
+        }
         double lum_b = 0, spec_b = 0, bg_b = 0;
         // the luminosity of channel c: (ambient + diff) (+ sh_c) (+ P_c)
         auto lum_of = [&](int c) {
@@ -1136,11 +1152,17 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 ? 1 : 0) k_phong_shade_b(
             }
         }
         acc[3] += lum_b;
+        double diff_b = lum_b;
+        if constexpr (SUN) {
+            sun_vis_b[p] = (float)(lum_b * diff0 + spec_b * spec0);
+            diff_b = __dmul_rn(lum_b, sv);
+            spec_b = __dmul_rn(spec_b, sv);
+        }
         double a_b = -bg_b, N_b[3] = {0, 0, 0}, X_b[3] = {0, 0, 0};
         if (t.lit && t.dot_nl < 0)
             for (int j = 0; j < 3; j++) {
-                n_b[j] -= lum_b * prm[j];
-                acc[j] -= lum_b * t.n[j];
+                n_b[j] -= diff_b * prm[j];
+                acc[j] -= diff_b * t.n[j];
             }
         if (t.spec_on) {
             a_b += spec_b * ((ks * t.ll) * t.p);
@@ -1369,15 +1391,18 @@ void launch_sh_lit_b(const double *normals, const double *vcol, int n, int C, co
                                                      sh_b, s);
 }
 
-template <int S, bool SPLIT = false>
+template <int S, bool SPLIT = false, bool SUN = false>
 void launch_phong_b(const DeodrPhongIO &io, const double *sh, double *sh_b, Scratch *s, cudaStream_t st,
-                    const float *albedo = nullptr, float *albedo_b = nullptr) {
+                    const float *albedo = nullptr, float *albedo_b = nullptr, const float *sun_vis = nullptr,
+                    float *sun_vis_b = nullptr) {
     const long long pixels = (long long)io.H * io.W;
     const int g = reduce_grid(pixels);
     if (io.camera_center_b)
-        k_phong_shade_b<true, S, SPLIT><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, nullptr, 0);
+        k_phong_shade_b<true, S, SPLIT, 0, false, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, nullptr, 0,
+                                                                         nullptr, nullptr, sun_vis, sun_vis_b);
     else
-        k_phong_shade_b<false, S, SPLIT><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, nullptr, 0);
+        k_phong_shade_b<false, S, SPLIT, 0, false, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, nullptr, 0,
+                                                                          nullptr, nullptr, sun_vis, sun_vis_b);
     if constexpr (S > 0)
         k_phong_sh_b<S, SPLIT><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo);
 }
@@ -1397,21 +1422,43 @@ void with_point_channels(int S, int P, F &&f) {
 #undef POINT_CASE
 }
 
+// Calls f(S) with S from 0 to 4 as a compile-time constant (S = 0: no environment)
+template <typename F>
+void with_sh_channels(int S, F &&f) {
+    switch (S) {
+        case 0: return f(std::integral_constant<int, 0>{});
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 2: return f(std::integral_constant<int, 2>{});
+        case 3: return f(std::integral_constant<int, 3>{});
+        default: return f(std::integral_constant<int, 4>{});
+    }
+}
+
+// Calls f(b) with b as a compile-time constant
+template <typename F>
+void with_flag(bool b, F &&f) {
+    if (b) return f(std::true_type{});
+    return f(std::false_type{});
+}
+
 // the grid of a (L lights) x (CTAs per light) light sum over `items` items: at most MAX_K * MAX_CTAS partials
 dim3 light_grid(long long items, int L, int P) {
     return dim3(L, std::max(1, std::min(reduce_grid(items), MAX_K * MAX_CTAS / (L * (3 + P)))));
 }
 
-template <int S, int P, bool SPLIT, bool VIS = false>
+template <int S, int P, bool SPLIT, bool VIS = false, bool SUN = false>
 void launch_point_phong_b(const DeodrPhongIO &io, const float *albedo, float *albedo_b, const double *sh,
                           double *sh_b, const double *lights, int L, double *lights_b, Scratch *s, cudaStream_t st,
-                          const float *vis = nullptr, float *vis_b = nullptr) {
+                          const float *vis = nullptr, float *vis_b = nullptr, const float *sun_vis = nullptr,
+                          float *sun_vis_b = nullptr) {
     const long long pixels = (long long)io.H * io.W;
     const int g = reduce_grid(pixels);
     if (io.camera_center_b)
-        k_phong_shade_b<true, S, SPLIT, P, VIS><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis, vis_b);
+        k_phong_shade_b<true, S, SPLIT, P, VIS, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis,
+                                                                       vis_b, sun_vis, sun_vis_b);
     else
-        k_phong_shade_b<false, S, SPLIT, P, VIS><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis, vis_b);
+        k_phong_shade_b<false, S, SPLIT, P, VIS, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis,
+                                                                        vis_b, sun_vis, sun_vis_b);
     if constexpr (S > 0)
         k_phong_sh_b<S, SPLIT><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo);
     k_point_lights_pixel_b<P, SPLIT, VIS><<<light_grid(pixels, L, P), NT, 0, st>>>(io, albedo, lights, lights_b, s,
@@ -1862,6 +1909,88 @@ int deodr_b200_point_phong_shade_shadowed_b(const DeodrPhongIO *io, const float 
         else
             launch_point_phong_b<S, P, false, true>(*io, nullptr, nullptr, sh, sh_b, lights, nb_lights, lights_b, s,
                                                     st, vis, vis_b);
+    });
+    return check_launch();
+}
+
+int deodr_b200_phong_shade_sun_shadowed(const DeodrPhongIO *io, const float *albedo, const double *sh,
+                                        int sh_channels, const double *lights, int nb_lights, int light_channels,
+                                        const float *vis, const float *sun_vis, void *stream) {
+    if (!phong_io_ok(io, albedo != nullptr) || !io->image || (!sh && sh_channels != 0) ||
+        (!lights && (nb_lights != 0 || vis)) || !sun_vis)
+        return bad("phong_shade_sun_shadowed: bad argument (H, W >= 1, C in [1, 32760], offsets tiling [0, C + 7), "
+                   "or [0, 7) with off_albedo -1 and an albedo, channels, params, camera_center, background, image "
+                   "and sun_vis non-NULL, sh NULL only with sh_channels 0, lights NULL only with nb_lights 0 and no "
+                   "vis)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) ||
+        (lights && (!light_channels_ok(light_channels, io->C) || nb_lights < 1 || nb_lights > MAX_LIGHTS)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "phong_shade_sun_shadowed: nb_lights must be 1 to 8, and "
+                                                  "sh_channels and light_channels 1, or C from 1 to 4");
+    const int g = grid_of((long long)io->H * io->W);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S_ = sh ? sh_channels : 0;
+    if (!lights) {
+        with_sh_channels(S_, [&](auto S) {
+            if (albedo)
+                k_phong_shade<S, true, 0, false, true><<<g, NT, 0, st>>>(*io, sh, albedo, nullptr, 0, nullptr,
+                                                                         sun_vis);
+            else
+                k_phong_shade<S, false, 0, false, true><<<g, NT, 0, st>>>(*io, sh, nullptr, nullptr, 0, nullptr,
+                                                                          sun_vis);
+        });
+        return check_launch();
+    }
+    with_point_channels(S_, light_channels, [&](auto S, auto P) {
+        with_flag(vis != nullptr, [&](auto VIS) {
+            if (albedo)
+                k_phong_shade<S, true, P, VIS, true><<<g, NT, 0, st>>>(*io, sh, albedo, lights, nb_lights, vis,
+                                                                       sun_vis);
+            else
+                k_phong_shade<S, false, P, VIS, true><<<g, NT, 0, st>>>(*io, sh, nullptr, lights, nb_lights, vis,
+                                                                        sun_vis);
+        });
+    });
+    return check_launch();
+}
+
+int deodr_b200_phong_shade_sun_shadowed_b(const DeodrPhongIO *io, const float *albedo, float *albedo_b,
+                                          const double *sh, int sh_channels, double *sh_b, const double *lights,
+                                          int nb_lights, int light_channels, double *lights_b, const float *vis,
+                                          float *vis_b, const float *sun_vis, float *sun_vis_b, double *scratch,
+                                          void *stream) {
+    if (!phong_io_ok(io, albedo != nullptr) || !io->image_b || !io->channels_b || !io->params_b ||
+        (albedo && !albedo_b) || (!sh && sh_channels != 0) || (sh && !sh_b) || (!lights && (nb_lights != 0 || vis)) ||
+        (lights && !lights_b) || (vis && !vis_b) || !sun_vis || !sun_vis_b || !scratch)
+        return bad("phong_shade_sun_shadowed_b: bad argument (H, W >= 1, C in [1, 32760], offsets tiling [0, C + 7), "
+                   "or [0, 7) with off_albedo -1 and an albedo, channels, params, camera_center, background, image_b, "
+                   "channels_b, params_b, sun_vis, sun_vis_b and scratch non-NULL, albedo_b non-NULL with an albedo, "
+                   "sh NULL only with sh_channels 0, sh_b non-NULL with sh, lights NULL only with nb_lights 0 and no "
+                   "vis, lights_b non-NULL with lights, vis_b non-NULL with vis)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) ||
+        (lights && (!light_channels_ok(light_channels, io->C) || nb_lights < 1 || nb_lights > MAX_LIGHTS)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "phong_shade_sun_shadowed_b: nb_lights must be 1 to 8, and "
+                                                  "sh_channels and light_channels 1, or C from 1 to 4");
+    Scratch *s = reinterpret_cast<Scratch *>(scratch);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S_ = sh ? sh_channels : 0;
+    if (!lights) {
+        with_sh_channels(S_, [&](auto S) {
+            if (albedo)
+                launch_phong_b<S, true, true>(*io, sh, sh_b, s, st, albedo, albedo_b, sun_vis, sun_vis_b);
+            else
+                launch_phong_b<S, false, true>(*io, sh, sh_b, s, st, nullptr, nullptr, sun_vis, sun_vis_b);
+        });
+        return check_launch();
+    }
+    with_point_channels(S_, light_channels, [&](auto S, auto P) {
+        with_flag(vis != nullptr, [&](auto VIS) {
+            if (albedo)
+                launch_point_phong_b<S, P, true, VIS, true>(*io, albedo, albedo_b, sh, sh_b, lights, nb_lights,
+                                                            lights_b, s, st, vis, vis_b, sun_vis, sun_vis_b);
+            else
+                launch_point_phong_b<S, P, false, VIS, true>(*io, nullptr, nullptr, sh, sh_b, lights, nb_lights,
+                                                             lights_b, s, st, vis, vis_b, sun_vis, sun_vis_b);
+        });
     });
     return check_launch();
 }

@@ -319,13 +319,59 @@ __global__ void __launch_bounds__(NT) k_cube_project_b(const double *points, int
         for (int k = threadIdx.x; k < K; k += NT) lights_b[(k / 3) * stride + k % 3] += tot[k];
 }
 
+// The soft 2x2 depth test of a point at map coordinates (u, v) and depth z, kept for the adjoint: the taps' texel
+// indices, their smoothstep tests s and derivatives ds, and the two lerps in fu.  Shared by the cube and sun maps.
+struct MapTaps {
+    double u, v, z, fu, fv, s[4], ds[4], top, bottom;
+    long long tap[4];  // texel indices, taps 00, 10, 01, 11
+};
+
 // The lookup of one surface point x in light p's cube map, kept for the adjoint.  valid: the projection is in front of
 // the face and finite (else V = 1).
-struct ShadowTap {
-    double cam[26], u, v, z, fu, fv, s[4], ds[4], top, bottom;
-    long long tap[4];  // texel indices into the light's six maps, taps 00, 10, 01, 11
+struct ShadowTap : MapTaps {
+    double cam[26];
     bool valid;
 };
+
+// V = lerp(lerp(s_00, s_10, fu), lerp(s_01, s_11, fu), fv) at (t.u, t.v, t.z) in the M x M map starting at texel
+// `base` of `maps`, s_k = s((D + bias - z) / softness + 1); indices clamped into [0, M)
+__device__ __forceinline__ double map_taps(MapTaps &t, int M, long long base, const float *maps, double bias,
+                                           double softness) {
+    const double u0 = floor(t.u), v0 = floor(t.v), top = M - 1.0;
+    t.fu = t.u - u0;
+    t.fv = t.v - v0;
+    const long long c0 = (long long)fmin(fmax(u0, 0.0), top), c1 = (long long)fmin(fmax(u0 + 1, 0.0), top);
+    const long long r0 = (long long)fmin(fmax(v0, 0.0), top), r1 = (long long)fmin(fmax(v0 + 1, 0.0), top);
+    t.tap[0] = base + r0 * M + c0;
+    t.tap[1] = base + r0 * M + c1;
+    t.tap[2] = base + r1 * M + c0;
+    t.tap[3] = base + r1 * M + c1;
+    for (int q = 0; q < 4; q++) {
+        const double y = (((double)maps[t.tap[q]] + bias) - t.z) / softness + 1.0;
+        const double yc = fmin(fmax(y, 0.0), 1.0);
+        t.s[q] = yc * yc * (3.0 - 2.0 * yc);
+        t.ds[q] = y > 0.0 && y < 1.0 ? 6.0 * yc * (1.0 - yc) : 0.0;
+    }
+    t.top = t.s[0] + t.fu * (t.s[1] - t.s[0]);
+    t.bottom = t.s[2] + t.fu * (t.s[3] - t.s[2]);
+    return t.top + t.fv * (t.bottom - t.top);
+}
+
+// The adjoint of map_taps from g = V_b: the texels' gradients into mb (fp32 atomics) and those of u, v and z
+__device__ __forceinline__ void map_taps_b(const MapTaps &t, double g, double softness, float *mb, double &fu_b,
+                                           double &fv_b, double &z_b) {
+    // V = top + fv (bottom - top), top / bottom = lerps in fu of the taps 00, 10 / 01, 11
+    const double top_b = g * (1.0 - t.fv), bottom_b = g * t.fv;
+    fv_b = g * (t.bottom - t.top);
+    fu_b = top_b * (t.s[1] - t.s[0]) + bottom_b * (t.s[3] - t.s[2]);
+    const double s_b[4] = {top_b * (1.0 - t.fu), top_b * t.fu, bottom_b * (1.0 - t.fu), bottom_b * t.fu};
+    z_b = 0;
+    for (int q = 0; q < 4; q++) {
+        const double D_b = s_b[q] * t.ds[q] / softness;
+        if (D_b != 0.0) atomicAdd(mb + t.tap[q], (float)D_b);
+        z_b -= D_b;
+    }
+}
 
 __device__ __forceinline__ double shadow_lookup(const double x[3], const double *p, int M, const float *maps,
                                                 double bias, double softness, ShadowTap &t) {
@@ -341,25 +387,7 @@ __device__ __forceinline__ double shadow_lookup(const double x[3], const double 
     t.v = ij[1];
     t.valid = t.z > 0 && isfinite(t.u) && isfinite(t.v);
     if (!t.valid) return 1.0;
-    const double u0 = floor(t.u), v0 = floor(t.v), top = M - 1.0;
-    t.fu = t.u - u0;
-    t.fv = t.v - v0;
-    const long long c0 = (long long)fmin(fmax(u0, 0.0), top), c1 = (long long)fmin(fmax(u0 + 1, 0.0), top);
-    const long long r0 = (long long)fmin(fmax(v0, 0.0), top), r1 = (long long)fmin(fmax(v0 + 1, 0.0), top);
-    const long long face = (long long)k * M * M;
-    t.tap[0] = face + r0 * M + c0;
-    t.tap[1] = face + r0 * M + c1;
-    t.tap[2] = face + r1 * M + c0;
-    t.tap[3] = face + r1 * M + c1;
-    for (int q = 0; q < 4; q++) {
-        const double y = (((double)maps[t.tap[q]] + bias) - t.z) / softness + 1.0;
-        const double yc = fmin(fmax(y, 0.0), 1.0);
-        t.s[q] = yc * yc * (3.0 - 2.0 * yc);
-        t.ds[q] = y > 0.0 && y < 1.0 ? 6.0 * yc * (1.0 - yc) : 0.0;
-    }
-    t.top = t.s[0] + t.fu * (t.s[1] - t.s[0]);
-    t.bottom = t.s[2] + t.fu * (t.s[3] - t.s[2]);
-    return t.top + t.fv * (t.bottom - t.top);
+    return map_taps(t, M, (long long)k * M * M, maps, bias, softness);
 }
 
 // vis [H,W,L] of the G-buffer's pixels, one thread per pixel (1 where a = 0)
@@ -410,18 +438,8 @@ __global__ void __launch_bounds__(NT) k_shadow_visibility_b(const float *ch, flo
             ShadowTap t;
             shadow_lookup(x, lights + j * lstride, M, maps + (long long)6 * j * M * M, bias, softness, t);
             if (!t.valid) continue;
-            // V = top + fv (bottom - top), top / bottom = lerps in fu of the taps 00, 10 / 01, 11
-            const double top_b = g * (1.0 - t.fv), bottom_b = g * t.fv;
-            const double fv_b = g * (t.bottom - t.top);
-            const double fu_b = top_b * (t.s[1] - t.s[0]) + bottom_b * (t.s[3] - t.s[2]);
-            const double s_b[4] = {top_b * (1.0 - t.fu), top_b * t.fu, bottom_b * (1.0 - t.fu), bottom_b * t.fu};
-            double z_b = 0;
-            float *mb = maps_b + (long long)6 * j * M * M;
-            for (int q = 0; q < 4; q++) {
-                const double D_b = s_b[q] * t.ds[q] / softness;
-                if (D_b != 0.0) atomicAdd(mb + t.tap[q], (float)D_b);
-                z_b -= D_b;
-            }
+            double fu_b, fv_b, z_b;
+            map_taps_b(t, g, softness, maps_b + (long long)6 * j * M * M, fu_b, fv_b, z_b);
             PointAdjoint pa;
             double v[3];
             project_point_b(load_cam(t.cam, 0), x, fu_b, fv_b, &z_b, 0, pa, v);
@@ -436,6 +454,181 @@ __global__ void __launch_bounds__(NT) k_shadow_visibility_b(const float *ch, flo
     }
     if (grid_sum<K>(acc, s, tot))
         for (int k = threadIdx.x; k < K; k += NT) lights_b[(k / 3) * lstride + k % 3] += tot[k];
+}
+
+// ---- the directional light's shadow map (the model of the sun shadow entry points, include/deodr_b200.h) ---------
+
+// Frisvad's orthonormal frame (e1, e2, d) around the direction d = l / |l| the light travels (d = +z where |l| = 0),
+// with a = 1 / (1 + d_z) away from the pole d_z < -0.9999999
+struct SunFrame {
+    double e1[3], e2[3], d[3], ll, a;
+    bool pole;
+};
+
+__device__ __forceinline__ void sun_frame(const double *l, SunFrame &f) {
+    f.ll = sqrt((l[0] * l[0] + l[1] * l[1]) + l[2] * l[2]);
+    for (int j = 0; j < 3; j++) f.d[j] = f.ll > 0 ? l[j] / f.ll : (j == 2 ? 1.0 : 0.0);
+    f.pole = f.d[2] < -0.9999999;
+    if (f.pole) {
+        f.a = 0;
+        f.e1[0] = 0; f.e1[1] = -1; f.e1[2] = 0;
+        f.e2[0] = -1; f.e2[1] = 0; f.e2[2] = 0;
+        return;
+    }
+    f.a = 1.0 / (1.0 + f.d[2]);
+    const double b = -f.d[0] * f.d[1] * f.a;
+    f.e1[0] = 1.0 - f.d[0] * f.d[0] * f.a; f.e1[1] = b; f.e1[2] = -f.d[0];
+    f.e2[0] = b; f.e2[1] = 1.0 - f.d[1] * f.d[1] * f.a; f.e2[2] = -f.d[1];
+}
+
+// l_b [3] from the gradients of e1, e2 and d: the frame's derivative, then (I - d d^T) / |l| (0 where |l| = 0)
+__device__ __forceinline__ void sun_frame_b(const SunFrame &f, const double *e1_b, const double *e2_b,
+                                            const double *d_in_b, double *l_b) {
+    double d_b[3] = {d_in_b[0], d_in_b[1], d_in_b[2]};
+    if (!(f.ll > 0)) {
+        l_b[0] = l_b[1] = l_b[2] = 0;
+        return;
+    }
+    if (!f.pole) {
+        const double a = f.a, x = f.d[0], y = f.d[1], B = e1_b[1] + e2_b[0];  // b = -x y a is e1_y and e2_x
+        d_b[0] += (-2.0 * x * a * e1_b[0] - y * a * B) - e1_b[2];
+        d_b[1] += (-x * a * B - 2.0 * y * a * e2_b[1]) - e2_b[2];
+        d_b[2] += a * a * ((x * x * e1_b[0] + x * y * B) + y * y * e2_b[1]);
+    }
+    const double dd = (f.d[0] * d_b[0] + f.d[1] * d_b[1]) + f.d[2] * d_b[2];
+    for (int j = 0; j < 3; j++) l_b[j] = (d_b[j] - f.d[j] * dd) / f.ll;
+}
+
+// The window of the map: its centre c, radius r and size M; k = phi / r, h = (M - 1) / 2
+struct SunWindow {
+    double c[3], r;
+    int M;
+};
+
+// (u, v, z) of a world point x and w = x - c: u = h + k <e1, w>, v = h + k <e2, w>, z = <d, w> + 2 r
+__device__ __forceinline__ void sun_point(const SunFrame &f, const SunWindow &win, const double *x, double w[3],
+                                          double &u, double &v, double &z) {
+    const double k = (0.5 * win.M - 2.0) / win.r, h = 0.5 * (win.M - 1);
+    for (int j = 0; j < 3; j++) w[j] = x[j] - win.c[j];
+    u = h + k * ((f.e1[0] * w[0] + f.e1[1] * w[1]) + f.e1[2] * w[2]);
+    v = h + k * ((f.e2[0] * w[0] + f.e2[1] * w[1]) + f.e2[2] * w[2]);
+    z = ((f.d[0] * w[0] + f.d[1] * w[1]) + f.d[2] * w[2]) + 2.0 * win.r;
+}
+
+// The adjoint of sun_point from (u_b, v_b, z_b): x_b, and the frame's gradients added into fb = (e1_b, e2_b, d_b)
+__device__ __forceinline__ void sun_point_b(const SunFrame &f, const SunWindow &win, const double w[3], double u_b,
+                                            double v_b, double z_b, double x_b[3], double fb[9]) {
+    const double k = (0.5 * win.M - 2.0) / win.r, ku = k * u_b, kv = k * v_b;
+    for (int j = 0; j < 3; j++) {
+        x_b[j] = (ku * f.e1[j] + kv * f.e2[j]) + z_b * f.d[j];
+        fb[j] += ku * w[j];
+        fb[3 + j] += kv * w[j];
+        fb[6 + j] += z_b * w[j];
+    }
+}
+
+__global__ void __launch_bounds__(NT) k_sun_project(const double *points, int n, const double *light, SunWindow win,
+                                                    double *ij, double *depths) {
+    const long long i = (long long)blockIdx.x * NT + threadIdx.x;
+    if (i >= n) return;
+    SunFrame f;
+    sun_frame(light, f);
+    double w[3];
+    sun_point(f, win, points + 3 * i, w, ij[2 * i], ij[2 * i + 1], depths[i]);
+}
+
+// grid_sum's 9 frame sums (e1_b, e2_b, d_b) taken through the frame's adjoint and added into light_b[0:3]
+__device__ __forceinline__ void sun_light_b(const double *light, const double (&acc)[9], Scratch *s, double *light_b) {
+    __shared__ double tot[9];
+    if (grid_sum<9>(acc, s, tot) && threadIdx.x == 0) {
+        SunFrame f;
+        sun_frame(light, f);
+        double l_b[3];
+        sun_frame_b(f, tot, tot + 3, tot + 6, l_b);
+        for (int j = 0; j < 3; j++) light_b[j] += l_b[j];
+    }
+}
+
+// The sun projection's adjoint from the rasteriser's ij_b [n,2] and depths_b [n] (fp32): vertices_b accumulated, one
+// thread per vertex (no atomics); light_b[0:3] through the frame, summed with grid_sum in a fixed order.  A vertex whose
+// upstream gradients are exactly 0 adds nothing.
+__global__ void __launch_bounds__(NT) k_sun_project_b(const double *points, int n, const double *light, SunWindow win,
+                                                      const float *ij_b, const float *depths_b, double *points_b,
+                                                      double *light_b, Scratch *s) {
+    double acc[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) acc[k] = 0;
+    SunFrame f;
+    sun_frame(light, f);
+    for (long long i = (long long)blockIdx.x * NT + threadIdx.x; i < n; i += (long long)gridDim.x * NT) {
+        const double gi = ij_b[2 * i], gj = ij_b[2 * i + 1], gd = depths_b[i];
+        if (gi == 0.0 && gj == 0.0 && gd == 0.0) continue;
+        double w[3], u, v, z, x_b[3];
+        sun_point(f, win, points + 3 * i, w, u, v, z);
+        sun_point_b(f, win, w, gi, gj, gd, x_b, acc);
+        for (int c = 0; c < 3; c++) points_b[3 * i + c] = DADD(points_b[3 * i + c], x_b[c]);
+    }
+    sun_light_b(light, acc, s, light_b);
+}
+
+// The lookup of one surface point x in the sun map: false (V = 1) where x is not finite, outside the window's sphere,
+// or the light is off
+__device__ __forceinline__ bool sun_lookup(const SunFrame &f, const SunWindow &win, const double x[3], double w[3],
+                                           MapTaps &t) {
+    if (!(f.ll > 0) || !isfinite(x[0]) || !isfinite(x[1]) || !isfinite(x[2])) return false;
+    sun_point(f, win, x, w, t.u, t.v, t.z);
+    return (w[0] * w[0] + w[1] * w[1]) + w[2] * w[2] <= win.r * win.r;
+}
+
+// sun_vis [H,W] of the G-buffer's pixels, one thread per pixel (1 where a = 0)
+__global__ void __launch_bounds__(NT) k_sun_visibility(const float *ch, long long pixels, int stride, int off_pos,
+                                                       int off_cov, const double *light, SunWindow win,
+                                                       const float *map, double bias, double softness, float *vis) {
+    const long long p = (long long)blockIdx.x * NT + threadIdx.x;
+    if (p >= pixels) return;
+    const float *px = ch + p * stride;
+    const double a = px[off_cov];
+    double V = 1.0;
+    if (a != 0.0) {
+        SunFrame f;
+        sun_frame(light, f);
+        const double x[3] = {px[off_pos] / a, px[off_pos + 1] / a, px[off_pos + 2] / a};
+        double w[3];
+        MapTaps t;
+        if (sun_lookup(f, win, x, w, t)) V = map_taps(t, win.M, 0, map, bias, softness);
+    }
+    vis[p] = (float)V;
+}
+
+// The sun visibility's adjoint from vis_b [H,W]: the taps' gradients (map_b, fp32 atomics) and x's, which goes into
+// the position and coverage slices of ch_b (accumulated) and through the projection into light_b[0:3] (grid_sum)
+__global__ void __launch_bounds__(NT) k_sun_visibility_b(const float *ch, float *ch_b, long long pixels, int stride,
+                                                         int off_pos, int off_cov, const double *light, SunWindow win,
+                                                         const float *map, double bias, double softness,
+                                                         const float *vis_b, float *map_b, double *light_b,
+                                                         Scratch *s) {
+    double acc[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) acc[k] = 0;
+    SunFrame f;
+    sun_frame(light, f);
+    for (long long p = (long long)blockIdx.x * NT + threadIdx.x; p < pixels; p += (long long)gridDim.x * NT) {
+        const float *px = ch + p * stride;
+        const double a = px[off_cov], g = vis_b[p];
+        if (a == 0.0 || g == 0.0) continue;
+        const double x[3] = {px[off_pos] / a, px[off_pos + 1] / a, px[off_pos + 2] / a};
+        double w[3];
+        MapTaps t;
+        if (!sun_lookup(f, win, x, w, t)) continue;
+        map_taps(t, win.M, 0, map, bias, softness);
+        double fu_b, fv_b, z_b, x_b[3];
+        map_taps_b(t, g, softness, map_b, fu_b, fv_b, z_b);
+        sun_point_b(f, win, w, fu_b, fv_b, z_b, x_b, acc);
+        float *pb = ch_b + p * stride;
+        for (int c = 0; c < 3; c++) pb[off_pos + c] = (float)((double)pb[off_pos + c] + x_b[c] / a);
+        pb[off_cov] = (float)((double)pb[off_cov] - ((x_b[0] * x[0] + x_b[1] * x[1]) + x_b[2] * x[2]) / a);
+    }
+    sun_light_b(light, acc, s, light_b);
 }
 
 // Calls f(L) with L from 1 to SHADOW_MAX_LIGHTS as a compile-time constant
@@ -462,6 +655,18 @@ int sum_grid(long long items, int K) {
 bool shadow_map_ok(int M) { return M >= 8 && M <= 4096; }
 bool shadow_band_ok(double bias, double softness) {
     return std::isfinite(bias) && std::isfinite(softness) && bias > 0 && softness > 0;
+}
+// the sun map's window: a finite centre and a finite radius > 0
+bool sun_window_ok(const double *center, double radius) {
+    return center && std::isfinite(center[0]) && std::isfinite(center[1]) && std::isfinite(center[2]) &&
+           std::isfinite(radius) && radius > 0;
+}
+SunWindow sun_window(const double *center, double radius, int M) {
+    SunWindow w;
+    for (int j = 0; j < 3; j++) w.c[j] = center[j];
+    w.r = radius;
+    w.M = M;
+    return w;
 }
 bool shadow_lights_ok(int L, int P) { return L >= 1 && L <= SHADOW_MAX_LIGHTS && P >= 1 && P <= 4; }
 
@@ -876,6 +1081,62 @@ int deodr_b200_shadow_visibility_b(const DeodrPhongIO *io, const double *lights,
             io->channels, io->channels_b, pixels, stride, io->off_position, io->off_coverage, lights,
             3 + light_channels, maps, map_size, bias, softness, vis_b, maps_b, lights_b, s);
     });
+    return check_launch();
+}
+
+int deodr_b200_sun_project(const double *vertices, int n, const double *light, const double *center, double radius,
+                           int map_size, double *ij, double *depths, void *stream) {
+    if (n < 1 || !vertices || !light || !ij || !depths || !shadow_map_ok(map_size) || !sun_window_ok(center, radius))
+        return set_error(DEODR_B200_EINVAL, "sun_project: bad argument (n >= 1, every pointer non-NULL, map_size in "
+                                            "[8, 4096], center finite, radius finite and > 0)");
+    k_sun_project<<<(unsigned)((n + NT - 1) / NT), NT, 0, (cudaStream_t)stream>>>(
+        vertices, n, light, sun_window(center, radius, map_size), ij, depths);
+    return check_launch();
+}
+
+int deodr_b200_sun_project_b(const double *vertices, int n, const double *light, const double *center, double radius,
+                             int map_size, const float *ij_b, const float *depths_b, double *vertices_b,
+                             double *light_b, double *scratch, void *stream) {
+    if (n < 1 || !vertices || !light || !ij_b || !depths_b || !vertices_b || !light_b || !scratch ||
+        !shadow_map_ok(map_size) || !sun_window_ok(center, radius))
+        return set_error(DEODR_B200_EINVAL, "sun_project_b: bad argument (n >= 1, every pointer non-NULL, map_size "
+                                            "in [8, 4096], center finite, radius finite and > 0)");
+    k_sun_project_b<<<sum_grid(n, 9), NT, 0, (cudaStream_t)stream>>>(
+        vertices, n, light, sun_window(center, radius, map_size), ij_b, depths_b, vertices_b, light_b,
+        reinterpret_cast<Scratch *>(scratch));
+    return check_launch();
+}
+
+int deodr_b200_sun_visibility(const DeodrPhongIO *io, const double *center, double radius, const float *map,
+                              int map_size, double bias, double softness, float *vis, void *stream) {
+    if (!shadow_io_ok(io) || !io->params || !map || !vis || !shadow_map_ok(map_size) ||
+        !shadow_band_ok(bias, softness) || !sun_window_ok(center, radius))
+        return set_error(DEODR_B200_EINVAL, "sun_visibility: bad argument (H, W >= 1, C in [1, 32760], position and "
+                                            "coverage offsets inside the G-buffer, every pointer non-NULL, map_size in "
+                                            "[8, 4096], bias, softness and radius finite and > 0, center finite)");
+    const long long pixels = (long long)io->H * io->W;
+    const int stride = io->off_albedo == -1 ? 7 : io->C + 7;
+    k_sun_visibility<<<(unsigned)((pixels + NT - 1) / NT), NT, 0, (cudaStream_t)stream>>>(
+        io->channels, pixels, stride, io->off_position, io->off_coverage, io->params,
+        sun_window(center, radius, map_size), map, bias, softness, vis);
+    return check_launch();
+}
+
+int deodr_b200_sun_visibility_b(const DeodrPhongIO *io, const double *center, double radius, const float *map,
+                                int map_size, double bias, double softness, const float *vis_b, float *map_b,
+                                double *light_b, double *scratch, void *stream) {
+    if (!shadow_io_ok(io) || !io->params || !io->channels_b || !map || !vis_b || !map_b || !light_b || !scratch ||
+        !shadow_map_ok(map_size) || !shadow_band_ok(bias, softness) || !sun_window_ok(center, radius))
+        return set_error(DEODR_B200_EINVAL, "sun_visibility_b: bad argument (H, W >= 1, C in [1, 32760], position "
+                                            "and coverage offsets inside the G-buffer, every pointer non-NULL, "
+                                            "map_size in [8, 4096], bias, softness and radius finite and > 0, center "
+                                            "finite)");
+    const long long pixels = (long long)io->H * io->W;
+    const int stride = io->off_albedo == -1 ? 7 : io->C + 7;
+    k_sun_visibility_b<<<sum_grid(pixels, 9), NT, 0, (cudaStream_t)stream>>>(
+        io->channels, io->channels_b, pixels, stride, io->off_position, io->off_coverage, io->params,
+        sun_window(center, radius, map_size), map, bias, softness, vis_b, map_b, light_b,
+        reinterpret_cast<Scratch *>(scratch));
     return check_launch();
 }
 

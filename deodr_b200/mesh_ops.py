@@ -426,7 +426,8 @@ def _phong_io(channels: torch.Tensor, params: torch.Tensor, center: torch.Tensor
 def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: torch.Tensor,
                 background: torch.Tensor, sh: Optional[torch.Tensor] = None,
                 albedo: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None,
-                visibility: Optional[torch.Tensor] = None) -> torch.Tensor:
+                visibility: Optional[torch.Tensor] = None,
+                sun_visibility: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The per-pixel shading of a G-buffer (deodr_b200_phong_shade, or deodr_b200_sh_phong_shade with ``sh``; model in
     include/deodr_b200.h): ``channels``
     [H,W,C+7] f32 laid out (albedo C, normal 3, position 3, coverage 1), ``params`` [6] fp64 on the device = (light
@@ -436,12 +437,25 @@ def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: tor
     then [H,W,7] = (normal, position, coverage) (deodr_b200_phong_shade_albedo).  ``point_lights``: a point-light
     table [L, 3 + S] fp64 on the device, in either form (deodr_b200_point_phong_shade).  ``visibility``: with point
     lights, the lights' visibility [H,W,L] f32 (:func:`shadow_visibility`), which multiplies each light's diffuse and
-    specular terms (deodr_b200_point_phong_shade_shadowed)."""
+    specular terms (deodr_b200_point_phong_shade_shadowed).  ``sun_visibility``: the directional light's visibility
+    [H,W] f32 (:func:`sun_visibility`), which multiplies its diffuse and specular terms, with or without an
+    environment, point lights and their ``visibility`` (deodr_b200_phong_shade_sun_shadowed)."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     H, W = keep[0].shape[:2]
     image = torch.empty((H, W, io.C), dtype=torch.float32, device=keep[0].device)
     io.image = image.data_ptr()
-    if visibility is not None:
+    if sun_visibility is not None:
+        sun = _check_sun_visibility(sun_visibility, H, W, image.device)
+        lights, L, P = _check_point_lights(point_lights, image.device) if point_lights is not None else (None, 0, 0)
+        vis = _check_visibility(visibility, H, W, L, image.device) if visibility is not None else None
+        if vis is not None and lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        sh, S = _check_sh(sh, image.device) if sh is not None else (None, 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        _cabi.check(_cabi.load().deodr_b200_phong_shade_sun_shadowed(
+            C.byref(io), ptr(keep[4]), ptr(sh), S, ptr(lights), L, P, ptr(vis), sun.data_ptr(),
+            _stream(image.device)))
+    elif visibility is not None:
         if point_lights is None:
             raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
         lights, L, P = _check_point_lights(point_lights, image.device)
@@ -475,7 +489,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
                          center_grad: bool = False, sh: Optional[torch.Tensor] = None,
                          albedo: Optional[torch.Tensor] = None,
                          point_lights: Optional[torch.Tensor] = None,
-                         visibility: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
+                         visibility: Optional[torch.Tensor] = None,
+                         sun_visibility: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
     """-> (channels_b [H,W,C+7] f32, params_b [6] fp64), the adjoint of :func:`phong_shade` from ``image_b`` [H,W,C]
     (deodr_b200_phong_shade_b, or deodr_b200_sh_phong_shade_b with ``sh``).  channels_b includes the coverage channel's gradient; ``params_b`` is summed over the
     pixels in a fixed order (bit-reproducible).  ``scratch``: a buffer of ``mesh_fitter.new_scratch``.  With
@@ -484,7 +499,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     :func:`phong_shade`; channels_b is then [H,W,7]) the result ends with albedo_b [H,W,C] f32
     (deodr_b200_phong_shade_albedo_b).  With ``point_lights`` the result ends with lights_b [L, 3 + S] fp64, summed
     in a fixed order (deodr_b200_point_phong_shade_b); with ``visibility`` too it then ends with vis_b [H,W,L] f32
-    (deodr_b200_point_phong_shade_shadowed_b)."""
+    (deodr_b200_point_phong_shade_shadowed_b).  With ``sun_visibility`` the result ends with sun_vis_b [H,W] f32
+    (deodr_b200_phong_shade_sun_shadowed_b)."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     dev = keep[0].device
     S = _check_sh(sh, dev)[1] if sh is not None else 0
@@ -503,8 +519,20 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
     if albedo is not None:
         albedo_b = torch.empty((H, W, io.C), dtype=torch.float32, device=dev)
-    lights_b = vis_b = None
-    if visibility is not None:
+    lights_b = vis_b = sun_b = None
+    if sun_visibility is not None:
+        sun = _check_sun_visibility(sun_visibility, H, W, dev)
+        lights, L, P = _check_point_lights(point_lights, dev) if point_lights is not None else (None, 0, 0)
+        vis = _check_visibility(visibility, H, W, L, dev) if visibility is not None else None
+        if vis is not None and lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        lights_b = torch.empty_like(lights) if lights is not None else None
+        vis_b = torch.empty((H, W, L), dtype=torch.float32, device=dev) if vis is not None else None
+        sun_b = torch.empty((H, W), dtype=torch.float32, device=dev)
+        _cabi.check(_cabi.load().deodr_b200_phong_shade_sun_shadowed_b(
+            C.byref(io), ptr(keep[4]), ptr(albedo_b), ptr(sh), S, ptr(sh_b), ptr(lights), L, P, ptr(lights_b),
+            ptr(vis), ptr(vis_b), sun.data_ptr(), sun_b.data_ptr(), scratch.data_ptr(), _stream(dev)))
+    elif visibility is not None:
         if point_lights is None:
             raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
         lights, L, P = _check_point_lights(point_lights, dev)
@@ -534,7 +562,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     out = out if sh_b is None else out + (sh_b,)
     out = out if albedo_b is None else out + (albedo_b,)
     out = out if lights_b is None else out + (lights_b,)
-    return out if vis_b is None else out + (vis_b,)
+    out = out if vis_b is None else out + (vis_b,)
+    return out if sun_b is None else out + (sun_b,)
 
 
 # ---- shadows from point lights (the model in include/deodr_b200.h) ---------------------------------------------------
@@ -667,6 +696,133 @@ def shadow_visibility_backward(channels: torch.Tensor, lights: torch.Tensor, map
         C.byref(io), lights.data_ptr(), L, S, maps.data_ptr(), M, float(bias), float(softness), vis_b.data_ptr(),
         maps_b.data_ptr(), lights_b.data_ptr(), scratch.data_ptr(), _stream(dev)))
     return channels_b, maps_b, lights_b
+
+
+# ---- shadows from the directional light (the model in include/deodr_b200.h) ------------------------------------------
+
+
+def _check_sun_visibility(vis: torch.Tensor, H: int, W: int, device) -> torch.Tensor:
+    if not isinstance(vis, torch.Tensor) or vis.dtype != torch.float32 or tuple(vis.shape) != (H, W) \
+            or not vis.is_contiguous() or vis.device != torch.device(device):
+        raise ValueError(f"sun_visibility must be a contiguous [{H},{W}] f32 tensor on {device}; got "
+                         f"{getattr(vis, 'dtype', type(vis))} {tuple(getattr(vis, 'shape', ()))}")
+    return vis
+
+
+def _check_sun_map(sun_map: torch.Tensor, device) -> Tuple[torch.Tensor, int]:
+    if not isinstance(sun_map, torch.Tensor) or sun_map.dtype != torch.float32 or sun_map.dim() != 2 \
+            or sun_map.shape[0] != sun_map.shape[1] or not sun_map.is_contiguous() \
+            or sun_map.device != torch.device(device):
+        raise ValueError(f"the sun map must be a contiguous [M, M] f32 tensor on {device}; got "
+                         f"{getattr(sun_map, 'dtype', type(sun_map))} {tuple(getattr(sun_map, 'shape', ()))}")
+    return sun_map, sun_map.shape[0]
+
+
+def _sun_bounds(bounds) -> Tuple[C.Array, float]:
+    """(centre as a C double[3], radius) of bounds (cx, cy, cz, r); the C entry points refuse bad values."""
+    b = [float(x) for x in bounds]
+    if len(b) != 4:
+        raise ValueError(f"bounds must be (cx, cy, cz, r); got {bounds!r}")
+    return (C.c_double * 3)(*b[:3]), b[3]
+
+
+def _light_vector(light: torch.Tensor, device) -> torch.Tensor:
+    """The directional light l [3] fp64 on ``device``: a [3] tensor, or the Phong params [6] whose first three it is."""
+    if not isinstance(light, torch.Tensor) or light.dtype != torch.float64 or light.dim() != 1 \
+            or light.shape[0] not in (3, 6) or not light.is_contiguous() or light.device != torch.device(device):
+        raise ValueError(f"light must be a contiguous [3] (or Phong params [6]) fp64 tensor on {device}; got "
+                         f"{getattr(light, 'dtype', type(light))} {tuple(getattr(light, 'shape', ()))}")
+    return light
+
+
+def sun_project(vertices: torch.Tensor, light: torch.Tensor, bounds, map_size: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The vertices [V,3] projected into the directional light's shadow map (deodr_b200_sun_project; the model in
+    include/deodr_b200.h) -> (ij [V,2], depths [V]) fp64.  ``light``: l [3] fp64 on the device (or the Phong params
+    [6]), read there; ``bounds``: the window (cx, cy, cz, r), host values."""
+    dev = vertices.device
+    vertices = _f64(vertices, dev)
+    light = _light_vector(light, dev)
+    center, radius = _sun_bounds(bounds)
+    n = vertices.shape[0]
+    ij = torch.empty((n, 2), dtype=torch.float64, device=dev)
+    depths = torch.empty((n,), dtype=torch.float64, device=dev)
+    _cabi.check(_cabi.load().deodr_b200_sun_project(vertices.data_ptr(), n, light.data_ptr(), center, radius,
+                                                    int(map_size), ij.data_ptr(), depths.data_ptr(), _stream(dev)))
+    return ij, depths
+
+
+def sun_project_backward(vertices: torch.Tensor, light: torch.Tensor, bounds, map_size: int, ij_b: torch.Tensor,
+                         depths_b: torch.Tensor, scratch: torch.Tensor, vertices_b: Optional[torch.Tensor] = None,
+                         light_b: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The adjoint of :func:`sun_project` from ``ij_b`` [V,2] and ``depths_b`` [V] (fp32, the rasteriser's) ->
+    (vertices_b [V,3], light_b [3] or [6]) fp64, accumulated into the given tensors (created zeroed if None; a
+    ``light_b`` of [6] takes the gradient in its first three entries), summed in a fixed order
+    (deodr_b200_sun_project_b).  ``scratch``: a buffer of ``mesh_fitter.new_scratch``."""
+    dev = vertices.device
+    vertices = _f64(vertices, dev)
+    light = _light_vector(light, dev)
+    center, radius = _sun_bounds(bounds)
+    n = vertices.shape[0]
+    ij_b = ij_b.to(device=dev, dtype=torch.float32).contiguous()
+    depths_b = depths_b.to(device=dev, dtype=torch.float32).contiguous()
+    if tuple(ij_b.shape) != (n, 2) or depths_b.numel() != n:
+        raise ValueError(f"ij_b must be [{n},2] and depths_b [{n}]; got {tuple(ij_b.shape)} and {tuple(depths_b.shape)}")
+    vertices_b = torch.zeros((n, 3), dtype=torch.float64, device=dev) if vertices_b is None else vertices_b
+    light_b = torch.zeros((3,), dtype=torch.float64, device=dev) if light_b is None else _light_vector(light_b, dev)
+    _cabi.check(_cabi.load().deodr_b200_sun_project_b(
+        vertices.data_ptr(), n, light.data_ptr(), center, radius, int(map_size), ij_b.data_ptr(), depths_b.data_ptr(),
+        vertices_b.data_ptr(), light_b.data_ptr(), scratch.data_ptr(), _stream(dev)))
+    return vertices_b, light_b
+
+
+def _sun_io(channels: torch.Tensor, light: torch.Tensor, albedo: Optional[torch.Tensor]):
+    io, channels = _shadow_io(channels, albedo)
+    io.params = _light_vector(light, channels.device).data_ptr()
+    return io, channels
+
+
+def sun_visibility(channels: torch.Tensor, light: torch.Tensor, sun_map: torch.Tensor, bounds, bias: float,
+                   softness: float, albedo: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The directional light's visibility [H,W] f32 of a Phong G-buffer's pixels (``channels`` [H,W,C+7], or [H,W,7]
+    beside a separate ``albedo``) under its shadow map ``sun_map`` [M,M] f32 (deodr_b200_sun_visibility; the model in
+    include/deodr_b200.h): ``light`` l [3] (or the Phong params [6]) fp64 on the device, ``bounds`` (cx, cy, cz, r),
+    ``bias`` and ``softness`` in world units.  1 where the coverage is 0, outside the bounds' sphere, or where l = 0."""
+    dev = channels.device
+    io, channels = _sun_io(channels, light, albedo)
+    sun_map, M = _check_sun_map(sun_map, dev)
+    center, radius = _sun_bounds(bounds)
+    vis = torch.empty((io.H, io.W), dtype=torch.float32, device=dev)
+    _cabi.check(_cabi.load().deodr_b200_sun_visibility(C.byref(io), center, radius, sun_map.data_ptr(), M, float(bias),
+                                                       float(softness), vis.data_ptr(), _stream(dev)))
+    return vis
+
+
+def sun_visibility_backward(channels: torch.Tensor, light: torch.Tensor, sun_map: torch.Tensor, bounds, bias: float,
+                            softness: float, vis_b: torch.Tensor, scratch: torch.Tensor,
+                            albedo: Optional[torch.Tensor] = None, channels_b: Optional[torch.Tensor] = None,
+                            map_b: Optional[torch.Tensor] = None,
+                            light_b: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
+    """The adjoint of :func:`sun_visibility` from ``vis_b`` [H,W] -> (channels_b, map_b [M,M] f32, light_b [3] or [6]
+    fp64), each accumulated into the given tensor (created zeroed if None; a ``light_b`` of [6], such as the shading's
+    params_b, takes the gradient in its first three entries): the position and coverage slices of channels_b, the
+    texels (fp32 atomics) and l, summed in a fixed order (deodr_b200_sun_visibility_b)."""
+    dev = channels.device
+    io, channels = _sun_io(channels, light, albedo)
+    sun_map, M = _check_sun_map(sun_map, dev)
+    center, radius = _sun_bounds(bounds)
+    vis_b = _check_sun_visibility(vis_b.to(dev, torch.float32).contiguous(), io.H, io.W, dev)
+    if channels_b is None:
+        channels_b = torch.zeros_like(channels)
+    if tuple(channels_b.shape) != tuple(channels.shape) or channels_b.dtype != torch.float32 \
+            or not channels_b.is_contiguous():
+        raise ValueError(f"channels_b must be a contiguous f32 tensor shaped like channels {tuple(channels.shape)}")
+    map_b = torch.zeros_like(sun_map) if map_b is None else map_b
+    light_b = torch.zeros((3,), dtype=torch.float64, device=dev) if light_b is None else _light_vector(light_b, dev)
+    io.channels_b = channels_b.data_ptr()
+    _cabi.check(_cabi.load().deodr_b200_sun_visibility_b(
+        C.byref(io), center, radius, sun_map.data_ptr(), M, float(bias), float(softness), vis_b.data_ptr(),
+        map_b.data_ptr(), light_b.data_ptr(), scratch.data_ptr(), _stream(dev)))
+    return channels_b, map_b, light_b
 
 
 def _light(light_directional):
@@ -984,19 +1140,44 @@ def check_shadow_arguments(shading: str, point_lights, size: int, bias, softness
     return size
 
 
-class ShadowCubes:
-    """The cube shadow maps of L point lights: 6L one-channel depth scenes of a mesh (face 6 j + k), whose ij, depths,
-    colours (the depth) and silhouette flags are slices of one buffer each, filled by one projection launch
-    (:func:`cube_project`) and one silhouette launch over a topology of 6L disjoint copies of the faces.  The caller
-    renders :attr:`scenes` beside its own in one renderer call, with :meth:`outputs` as their results, and
-    back-propagates them in one call with :meth:`image_bs` and :meth:`grads`, then calls :meth:`backward`."""
+def check_sun_shadow_arguments(shading: str, light_directional, size: int, bias, softness, bounds) -> int:
+    """The refusals of a view's (or a scene's) directional-light shadow arguments -> the map size M (0: none)."""
+    size = int(size)
+    if size == 0:
+        return 0
+    if shading not in ("phong", "phong_textured"):
+        raise ValueError("light shadows need per-pixel shading (shading='phong' or 'phong_textured'): a shadow edge "
+                         "crosses triangles, and per-vertex visibility would smear it over each one")
+    if light_directional is None:
+        raise ValueError("light shadows are cast from the directional light: this view has none")
+    if not SHADOW_MAP_SIZES[0] <= size <= SHADOW_MAP_SIZES[1]:
+        raise ValueError(f"light_shadow_map_size must be 0 or lie in [{SHADOW_MAP_SIZES[0]}, {SHADOW_MAP_SIZES[1]}]; "
+                         f"got {size}")
+    if bias is None or softness is None or bounds is None:
+        raise ValueError("light shadows need light_shadow_bias, light_shadow_softness and light_shadow_bounds (world "
+                         "units: the light has no position, so no default is free of scale)")
+    if not (np.isfinite(bias) and np.isfinite(softness) and bias > 0 and softness > 0):
+        raise ValueError(f"light_shadow_bias and light_shadow_softness must be finite and > 0; got {bias} and "
+                         f"{softness}")
+    b = np.asarray(bounds, dtype=np.float64).reshape(-1)
+    if b.shape != (4,) or not np.all(np.isfinite(b)) or not b[3] > 0:
+        raise ValueError(f"light_shadow_bounds must be (cx, cy, cz, r), finite, with r > 0; got {bounds!r}")
+    return size
 
-    def __init__(self, faces_u32: np.ndarray, V: int, L: int, M: int, clockwise: bool, device):
+
+class DepthMaps:
+    """NF one-channel M x M depth scenes of a mesh (the shadow maps), whose ij, depths, colours (the depth) and
+    silhouette flags are slices of one buffer each, filled by one projection launch and one silhouette launch over a
+    topology of NF disjoint copies of the faces.  The caller renders :attr:`scenes` beside its own in one renderer
+    call, with :meth:`outputs` as their results, and back-propagates them in one call with :meth:`image_bs` and
+    :meth:`grads`, then calls the subclass's ``backward``."""
+
+    def __init__(self, faces_u32: np.ndarray, V: int, NF: int, M: int, clockwise: bool, device):
         from .renderer import DeviceScene
         from .scenes import SceneArrays
 
-        T, NF = faces_u32.shape[0], 6 * L
-        self.L, self.M, self.V, self.device = L, M, V, device
+        T = faces_u32.shape[0]
+        self.NF, self.M, self.V, self.device = NF, M, V, device
         tiled = (faces_u32[None].astype(np.int64) + (np.arange(NF) * V)[:, None, None]).reshape(-1, 3)
         self.topology = MeshTopology(tiled, NF * V, clockwise=clockwise, device=device)
         self.edgeflags = torch.zeros((NF * T, 3), dtype=torch.uint8, device=device)
@@ -1030,12 +1211,9 @@ class ShadowCubes:
                           "barycentric": None, "err_buffer": None} for f in range(NF)]
         self._unused_b = base.zero_grads()
 
-    def prepare(self, vertices: torch.Tensor, lights: torch.Tensor) -> None:
-        """Projects the vertices through the cube cameras of ``lights`` (read on the device) and sets the scenes'
-        ij, depths, colours and silhouette flags."""
-        if lights.shape[0] != self.L:
-            raise ValueError(f"the view's shadow maps were made for {self.L} lights; the table has {lights.shape[0]}")
-        self.cameras, self.ij, self.depths = cube_project(vertices, lights, self.M)
+    def _set_projection(self, ij: torch.Tensor, depths: torch.Tensor) -> None:
+        """Sets the scenes' ij [NF, V, 2], depths [NF, V], colours and silhouette flags."""
+        self.ij, self.depths = ij, depths
         self.colors.copy_(self.depths[:, :, None])
         self.topology.edge_on_silhouette(self.ij.view(-1, 2), out=self.edgeflags)
         for f, sc in enumerate(self.scenes):
@@ -1049,7 +1227,7 @@ class ShadowCubes:
         return self.maps_b
 
     def image_bs(self, maps_b: torch.Tensor):
-        return [maps_b[f].view(self.M, self.M, 1) for f in range(6 * self.L)]
+        return [maps_b[f].view(self.M, self.M, 1) for f in range(self.NF)]
 
     def grads(self):
         """The faces' gradient slots: ij_b and colors_b slices of one buffer each, zeroed."""
@@ -1057,7 +1235,23 @@ class ShadowCubes:
         self.colors_b.zero_()
         u = self._unused_b
         return [{"ij_b": self.ij_b[f], "colors_b": self.colors_b[f], "uv_b": u["uv_b"], "shade_b": u["shade_b"],
-                 "texture_b": u["texture_b"]} for f in range(6 * self.L)]
+                 "texture_b": u["texture_b"]} for f in range(self.NF)]
+
+
+class ShadowCubes(DepthMaps):
+    """The cube shadow maps of L point lights: 6L depth scenes (face 6 j + k) projected by :func:`cube_project`."""
+
+    def __init__(self, faces_u32: np.ndarray, V: int, L: int, M: int, clockwise: bool, device):
+        super().__init__(faces_u32, V, 6 * L, M, clockwise, device)
+        self.L = L
+
+    def prepare(self, vertices: torch.Tensor, lights: torch.Tensor) -> None:
+        """Projects the vertices through the cube cameras of ``lights`` (read on the device) and sets the scenes'
+        ij, depths, colours and silhouette flags."""
+        if lights.shape[0] != self.L:
+            raise ValueError(f"the view's shadow maps were made for {self.L} lights; the table has {lights.shape[0]}")
+        self.cameras, ij, depths = cube_project(vertices, lights, self.M)
+        self._set_projection(ij, depths)
 
     def backward(self, vertices: torch.Tensor, lights: torch.Tensor, vertices_b: torch.Tensor,
                  lights_b: torch.Tensor, scratch: torch.Tensor) -> None:
@@ -1065,6 +1259,32 @@ class ShadowCubes:
         depth), accumulated into vertices_b and the positions of lights_b."""
         cube_project_backward(vertices, lights, self.M, self.cameras, self.ij_b, self.colors_b.view(6 * self.L, -1),
                               scratch, vertices_b=vertices_b, lights_b=lights_b)
+
+
+class SunShadowMap(DepthMaps):
+    """The directional light's shadow map: one depth scene projected by :func:`sun_project` over the window
+    ``bounds`` (cx, cy, cz, r)."""
+
+    def __init__(self, faces_u32: np.ndarray, V: int, M: int, bounds, clockwise: bool, device):
+        super().__init__(faces_u32, V, 1, M, clockwise, device)
+        self.bounds = tuple(float(b) for b in bounds)
+
+    @property
+    def map(self) -> torch.Tensor:
+        return self.maps[0]
+
+    def prepare(self, vertices: torch.Tensor, light: torch.Tensor) -> None:
+        """Projects the vertices into the map of ``light`` (l [3] or the Phong params [6], read on the device) and
+        sets the scene's ij, depths, colour and silhouette flags."""
+        ij, depths = sun_project(vertices, light, self.bounds, self.M)
+        self._set_projection(ij[None], depths[None])
+
+    def backward(self, vertices: torch.Tensor, light: torch.Tensor, vertices_b: torch.Tensor, light_b: torch.Tensor,
+                 scratch: torch.Tensor) -> None:
+        """The projection's adjoint after the map's raster adjoint, accumulated into vertices_b and light_b (l's
+        gradient: [3], or the Phong params_b [6])."""
+        sun_project_backward(vertices, light, self.bounds, self.M, self.ij_b[0], self.colors_b.view(-1), scratch,
+                             vertices_b=vertices_b, light_b=light_b)
 
 
 class DeviceMeshView:
@@ -1127,7 +1347,18 @@ class DeviceMeshView:
     :meth:`backward` adds the shadows' share to ``vertices_b`` (occluders and receivers) and to the lights' positions
     in ``point_lights_b``; the camera's gradient has none (the lookup does not read the camera).  Gouraud views refuse
     shadows: a shadow edge crosses triangles, and per-vertex visibility would smear it over each one.
-    :meth:`shadow_maps` returns the last maps."""
+    :meth:`shadow_maps` returns the last maps.
+
+    ``light_shadow_map_size`` M > 0 makes the directional light cast shadows in a Phong or textured Phong view (the
+    model in include/deodr_b200.h): one orthographic M x M depth map of the mesh, seen along the light's direction
+    over the window ``light_shadow_bounds`` = (cx, cy, cz, r), with the soft 2x2 test of the cube maps set by
+    ``light_shadow_bias`` and ``light_shadow_softness`` (bias, softness and bounds in world units, all required: the
+    light has no position, so no default is free of scale).  The directional diffuse and specular terms are
+    multiplied by it; receivers outside the bounds' sphere are lit.  The map is rendered and back-propagated in the
+    same renderer calls as the view's raster(s) and any cube faces, and :meth:`backward` adds the shadow's share to
+    ``vertices_b`` and to the light's direction in ``light_b[0:3]``.  The view needs a directional light, and Gouraud
+    views refuse it.  :meth:`light_shadow_map` and :meth:`light_shadow_visibility` return the last map and
+    visibility."""
 
     def __init__(self, faces, nb_vertices: int, camera, height: int, width: int, renderer=None,
                  light_directional=None, ambient: float = 1.0, background_color=(0.0, 0.0, 0.0), sigma: float = 1.0,
@@ -1136,7 +1367,9 @@ class DeviceMeshView:
                  specular: float = 0.0, shininess: float = 16.0, has_distortion: bool = True,
                  sh: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None,
                  shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
-                 shadow_softness: Optional[float] = None):
+                 shadow_softness: Optional[float] = None, light_shadow_map_size: int = 0,
+                 light_shadow_bias: Optional[float] = None, light_shadow_softness: Optional[float] = None,
+                 light_shadow_bounds=None):
         from .renderer import DeviceScene, default_renderer
         from .scenes import SceneArrays
 
@@ -1174,6 +1407,13 @@ class DeviceMeshView:
                                                       shadow_softness)
         self.shadow_bias = float(shadow_bias) if self.shadow_map_size else None
         self.shadow_softness = float(shadow_softness) if self.shadow_map_size else None
+        self.light_shadow_map_size = check_sun_shadow_arguments(shading, light_directional, light_shadow_map_size,
+                                                                light_shadow_bias, light_shadow_softness,
+                                                                light_shadow_bounds)
+        sun = self.light_shadow_map_size
+        self.light_shadow_bias = float(light_shadow_bias) if sun else None
+        self.light_shadow_softness = float(light_shadow_softness) if sun else None
+        self.light_shadow_bounds = tuple(float(b) for b in light_shadow_bounds) if sun else None
         self._sh_scratch, self._sh_key = None, None
         if textured:
             if uv is None or faces_uv is None or texture is None:
@@ -1244,8 +1484,14 @@ class DeviceMeshView:
             self._phong_scratch = new_scratch(self.device)
             self._phong_key = None
             self._phong_background = torch.from_numpy(background.astype(np.float32)).to(self.device)
+        self._maps = []  # the shadow maps rendered beside the view's raster(s): the cube maps, then the sun map
         if self.shadow_map_size:
             self._cube = ShadowCubes(faces_u32, V, point_lights.shape[0], self.shadow_map_size, clockwise, self.device)
+            self._maps.append(self._cube)
+        if self.light_shadow_map_size:
+            self._sun = SunShadowMap(faces_u32, V, self.light_shadow_map_size, self.light_shadow_bounds, clockwise,
+                                     self.device)
+            self._maps.append(self._sun)
 
     def _new_outputs(self, scene) -> dict:
         return self.renderer._new_outputs(scene, False, False, False)
@@ -1261,31 +1507,95 @@ class DeviceMeshView:
         """The lights' visibility [H,W,L] f32 of the last render's pixels (1 where the coverage is 0)."""
         if not self.shadow_map_size:
             raise ValueError("this view casts no shadows (shadow_map_size 0)")
+        return self._saved[-2]
+
+    def light_shadow_map(self) -> torch.Tensor:
+        """The directional light's shadow map [M, M] f32 of the last render (overwritten by the next render)."""
+        if not self.light_shadow_map_size:
+            raise ValueError("the directional light casts no shadows in this view (light_shadow_map_size 0)")
+        return self._sun.map
+
+    def light_shadow_visibility(self) -> torch.Tensor:
+        """The directional light's visibility [H,W] f32 of the last render's pixels (1 where the coverage is 0)."""
+        if not self.light_shadow_map_size:
+            raise ValueError("the directional light casts no shadows in this view (light_shadow_map_size 0)")
         return self._saved[-1]
+
+    def _render_with_maps(self, scenes: list, vertices: torch.Tensor, params: torch.Tensor) -> list:
+        """The view's scenes and every shadow map in one renderer call (one live forward per slot) -> the scenes'
+        forward results; the maps keep theirs."""
+        if not self._maps:
+            return self.renderer.render_views(scenes, self.sigma) if len(scenes) > 1 else \
+                [self.renderer.render(scenes[0], self.sigma)]
+        if self.shadow_map_size:
+            self._cube.prepare(vertices, self.point_lights)
+        if self.light_shadow_map_size:
+            self._sun.prepare(vertices, params)
+        fwds = self.renderer.render_views(scenes + [sc for m in self._maps for sc in m.scenes], self.sigma,
+                                          out=[self._new_outputs(sc) for sc in scenes]
+                                          + [o for m in self._maps for o in m.outputs()])
+        k = len(scenes)
+        for m in self._maps:
+            m.fwds, k = fwds[k:k + m.NF], k + m.NF
+        return fwds[:len(scenes)]
+
+    def _render_b_with_maps(self, scenes: list, fwds: list, image_bs: list, maps_bs: list) -> list:
+        """The adjoint of :meth:`_render_with_maps` in one renderer call -> the scenes' gradients."""
+        if not self._maps:
+            if len(scenes) == 1:
+                return [self.renderer.render_b(scenes[0], self.sigma, fwds[0], image_bs[0])]
+            return self.renderer.render_b_views(scenes, self.sigma, fwds, image_bs)
+        grads = self.renderer.render_b_views(
+            scenes + [sc for m in self._maps for sc in m.scenes], self.sigma,
+            list(fwds) + [f for m in self._maps for f in m.fwds],
+            list(image_bs) + [b for m, mb in zip(self._maps, maps_bs) for b in m.image_bs(mb)],
+            [sc.zero_grads() for sc in scenes] + [g for m in self._maps for g in m.grads()])
+        return grads[:len(scenes)]
+
+    def _maps_backward(self, vertices: torch.Tensor, params: torch.Tensor, vertices_b: torch.Tensor,
+                       params_b: torch.Tensor, lights_b: Optional[torch.Tensor]) -> None:
+        """The shadow maps' projection adjoints into vertices_b, the point lights' positions and l = params_b[0:3]."""
+        if self.shadow_map_size:
+            self._cube.backward(vertices, self.point_lights, vertices_b, lights_b, self._phong_scratch)
+        if self.light_shadow_map_size:
+            self._sun.backward(vertices, params, vertices_b, params_b, self._phong_scratch)
 
     def _shade(self, gbuffer: torch.Tensor, params: torch.Tensor, center: torch.Tensor, background: torch.Tensor,
                albedo: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
-        """phong_shade of a G-buffer, under the lights' visibility in a view with shadows -> (image, vis or None)."""
-        vis = None
+        """phong_shade of a G-buffer, under the point lights' and the directional light's visibility in a view with
+        shadows -> (image, vis or None, sun_vis or None)."""
+        vis = sun_vis = None
         if self.shadow_map_size:
             vis = shadow_visibility(gbuffer, self.point_lights, self._cube.maps, self.shadow_bias,
                                     self.shadow_softness, albedo=albedo)
+        if self.light_shadow_map_size:
+            sun_vis = sun_visibility(gbuffer, params, self._sun.map, self.light_shadow_bounds, self.light_shadow_bias,
+                                     self.light_shadow_softness, albedo=albedo)
         return phong_shade(gbuffer, params, center, background, sh=self.sh, albedo=albedo,
-                           point_lights=self.point_lights, visibility=vis), vis
+                           point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis), vis, sun_vis
 
-    def _shade_backward(self, gbuffer, params, center, background, image_b, camera_grad, albedo, vis):
-        """phong_shade_backward, and in a view with shadows the visibility's adjoint added into channels_b and lights_b
-        -> (the result of phong_shade_backward without vis_b, the cube maps' gradient [6L, M, M] or None)."""
+    def _shade_backward(self, gbuffer, params, center, background, image_b, camera_grad, albedo, vis, sun_vis):
+        """phong_shade_backward, and in a view with shadows the visibilities' adjoints added into channels_b, lights_b
+        and params_b -> (the result of phong_shade_backward without vis_b and sun_vis_b, the maps' gradients in the
+        order of self._maps)."""
         shaded = phong_shade_backward(gbuffer, params, center, background, image_b, self._phong_scratch,
                                       center_grad=camera_grad, sh=self.sh, albedo=albedo,
-                                      point_lights=self.point_lights, visibility=vis)
-        if vis is None:
-            return shaded, None
-        shaded, vis_b = shaded[:-1], shaded[-1]
-        _, maps_b, _ = shadow_visibility_backward(gbuffer, self.point_lights, self._cube.maps, self.shadow_bias,
-                                                  self.shadow_softness, vis_b, self._phong_scratch, albedo=albedo,
-                                                  channels_b=shaded[0], maps_b=self._cube.zero_maps_b(),
-                                                  lights_b=shaded[-1])
+                                      point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis)
+        maps_b = []
+        sun_b = None
+        if sun_vis is not None:
+            shaded, sun_b = shaded[:-1], shaded[-1]
+        if vis is not None:
+            shaded, vis_b = shaded[:-1], shaded[-1]
+            maps_b.append(shadow_visibility_backward(gbuffer, self.point_lights, self._cube.maps, self.shadow_bias,
+                                                     self.shadow_softness, vis_b, self._phong_scratch, albedo=albedo,
+                                                     channels_b=shaded[0], maps_b=self._cube.zero_maps_b(),
+                                                     lights_b=shaded[-1])[1])
+        if sun_b is not None:
+            maps_b.append(sun_visibility_backward(gbuffer, params, self._sun.map, self.light_shadow_bounds,
+                                                  self.light_shadow_bias, self.light_shadow_softness, sun_b,
+                                                  self._phong_scratch, albedo=albedo, channels_b=shaded[0],
+                                                  map_b=self._sun.zero_maps_b()[0], light_b=shaded[1])[1][None])
         return shaded, maps_b
 
     def _phong_params(self) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -1411,18 +1721,10 @@ class DeviceMeshView:
         t["colors"][:, nc:nc + 3].copy_(normals)
         t["colors"][:, nc + 3:nc + 6].copy_(vertices)
         self.topology.edge_on_silhouette(ij, out=t["edgeflags"])
-        if self.shadow_map_size:
-            # the G-buffer and the 6L cube faces in one call (one live forward per slot)
-            self._cube.prepare(vertices, self.point_lights)
-            fwds = self.renderer.render_views([self._phong_scene] + self._cube.scenes, self.sigma,
-                                              out=[self._new_outputs(self._phong_scene)] + self._cube.outputs())
-            fwd = fwds[0]
-            self._cube.fwds = fwds[1:]
-        else:
-            fwd = self.renderer.render(self._phong_scene, self.sigma)
         params, center = self._phong_params()
-        image, vis = self._shade(fwd["image"], params, center, self.scene.t["background_color"])
-        self._saved = (vertices, vertex_colors, normals, fwd, params, center, vis)
+        fwd = self._render_with_maps([self._phong_scene], vertices, params)[0]
+        image, vis, sun_vis = self._shade(fwd["image"], params, center, self.scene.t["background_color"])
+        self._saved = (vertices, vertex_colors, normals, fwd, params, center, vis, sun_vis)
         return image
 
     def _backward_phong(self, image_b: torch.Tensor, reference_transpose: bool,
@@ -1430,25 +1732,19 @@ class DeviceMeshView:
         # phong_shade_b -> channels_b; raster adjoint -> colors_b [V,K], ij_b; the albedo slice is vertex_colors_b, the
         # normal slice goes through the normal adjoint, the position slice adds to vertices_b, ij_b through the
         # projection's adjoint
-        vertices, _, _, fwd, params, center, vis = self._saved
+        vertices, _, _, fwd, params, center, vis, sun_vis = self._saved
         nc = self.scene.nb_colors
         shaded, maps_b = self._shade_backward(fwd["image"], params, center, self.scene.t["background_color"], image_b,
-                                              camera_grad, None, vis)
+                                              camera_grad, None, vis, sun_vis)
         lights_b = None
         if self.point_lights is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
         channels_b, params_b = shaded[:2]
-        if maps_b is not None:
-            grads = self.renderer.render_b_views([self._phong_scene] + self._cube.scenes, self.sigma,
-                                                 [fwd] + self._cube.fwds, [channels_b] + self._cube.image_bs(maps_b),
-                                                 [self._phong_scene.zero_grads()] + self._cube.grads())[0]
-        else:
-            grads = self.renderer.render_b(self._phong_scene, self.sigma, fwd, channels_b)
+        grads = self._render_b_with_maps([self._phong_scene], [fwd], [channels_b], maps_b)[0]
         colors_b = grads["colors_b"]
         vertices_b = self.topology.vertex_normals_backward(vertices, colors_b[:, nc:nc + 3])
         vertices_b += colors_b[:, nc + 3:nc + 6]
-        if maps_b is not None:
-            self._cube.backward(vertices, self.point_lights, vertices_b, lights_b, self._phong_scratch)
+        self._maps_backward(vertices, params, vertices_b, params_b, lights_b)
         _, camera_b = self._project_backward(vertices, grads["ij_b"], None, vertices_b, reference_transpose,
                                              camera_grad)
         out = {"vertices_b": vertices_b, "vertex_colors_b": colors_b[:, :nc].to(torch.float64),
@@ -1483,17 +1779,11 @@ class DeviceMeshView:
         g["colors"][:, 3:6].copy_(vertices)
         self.topology.edge_on_silhouette(ij, out=a["edgeflags"])
         g["edgeflags"].copy_(a["edgeflags"])
-        if self.shadow_map_size:
-            self._cube.prepare(vertices, self.point_lights)
-            fwds = self.renderer.render_views([self.scene, self._phong_scene] + self._cube.scenes, self.sigma,
-                                              out=[self._new_outputs(self.scene), self._new_outputs(self._phong_scene)]
-                                              + self._cube.outputs())
-            fwds, self._cube.fwds = fwds[:2], fwds[2:]
-        else:
-            fwds = self.renderer.render_views([self.scene, self._phong_scene], self.sigma)
         params, center = self._phong_params()
-        image, vis = self._shade(fwds[1]["image"], params, center, self._phong_background, albedo=fwds[0]["image"])
-        self._saved = (vertices, None, normals, fwds, params, center, vis)
+        fwds = self._render_with_maps([self.scene, self._phong_scene], vertices, params)
+        image, vis, sun_vis = self._shade(fwds[1]["image"], params, center, self._phong_background,
+                                          albedo=fwds[0]["image"])
+        self._saved = (vertices, None, normals, fwds, params, center, vis, sun_vis)
         return image
 
     def _backward_phong_textured(self, image_b: torch.Tensor, reference_transpose: bool,
@@ -1501,26 +1791,18 @@ class DeviceMeshView:
         # the shading's adjoint -> albedo_b, channels_b; one adjoint call over both rasters -> texture_b, uv_b and the
         # G-buffer's colors_b (normal slice through the normal adjoint, position slice into vertices_b); the two ij_b
         # are summed before the projection's adjoint.  The albedo raster's shade_b is not used: its shade is constant
-        vertices, _, _, fwds, params, center, vis = self._saved
+        vertices, _, _, fwds, params, center, vis, sun_vis = self._saved
         shaded, maps_b = self._shade_backward(fwds[1]["image"], params, center, self._phong_background, image_b,
-                                              camera_grad, fwds[0]["image"], vis)
+                                              camera_grad, fwds[0]["image"], vis, sun_vis)
         lights_b = None
         if self.point_lights is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
         channels_b, params_b, albedo_b = shaded[0], shaded[1], shaded[-1]
-        if maps_b is not None:
-            ga, gg = self.renderer.render_b_views(
-                [self.scene, self._phong_scene] + self._cube.scenes, self.sigma, list(fwds) + self._cube.fwds,
-                [albedo_b, channels_b] + self._cube.image_bs(maps_b),
-                [self.scene.zero_grads(), self._phong_scene.zero_grads()] + self._cube.grads())[:2]
-        else:
-            ga, gg = self.renderer.render_b_views([self.scene, self._phong_scene], self.sigma, fwds,
-                                                  [albedo_b, channels_b])
+        ga, gg = self._render_b_with_maps([self.scene, self._phong_scene], fwds, [albedo_b, channels_b], maps_b)
         colors_b = gg["colors_b"]
         vertices_b = self.topology.vertex_normals_backward(vertices, colors_b[:, 0:3])
         vertices_b += colors_b[:, 3:6]
-        if maps_b is not None:
-            self._cube.backward(vertices, self.point_lights, vertices_b, lights_b, self._phong_scratch)
+        self._maps_backward(vertices, params, vertices_b, params_b, lights_b)
         _, camera_b = self._project_backward(vertices, ga["ij_b"] + gg["ij_b"], None, vertices_b,
                                              reference_transpose, camera_grad)
         out = {"vertices_b": vertices_b, "texture_b": ga["texture_b"], "uv_b": ga["uv_b"], "light_b": params_b[:4],

@@ -39,6 +39,9 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
                            and one adjoint call; the maps' share reaches the vertices and the lights' positions
     ShadowVisibilityFunc   (G-buffer, point_lights, maps, bias, softness, albedo | None) -> visibility [H,W,L]; the
                            G-buffer, the maps and the lights' positions receive their gradients
+    SunVisibilityFunc      (G-buffer, light_directional [3], map [M,M], bounds, bias, softness, albedo | None) ->
+                           visibility [H,W] of the directional light; the G-buffer, the map and the light receive
+                           their gradients
 
 All maths is fp64 but the rasteriser's (fp32 image and image gradients).  ``RenderMesh2DFunc``,
 ``RenderMesh2DTexturedFunc`` and ``RenderMeshPhongTexturedFunc`` follow the snapshot / replay rule of the 2D Functions (differentiable_renderer_pytorch.py):
@@ -55,7 +58,9 @@ import torch
 
 from ..mesh_fitter import DeviceLaplacianRigidEnergy, new_scratch, pose, pose_backward
 from ..mesh_ops import (CameraParams, LoopSubdivision, MeshTopology, camera_center, lit_vertex_colors,
-                        ShadowCubes, check_shadow_arguments, cube_project_backward, lit_vertex_colors_backward,
+                        ShadowCubes, SunShadowMap, check_shadow_arguments, check_sun_shadow_arguments,
+                        cube_project_backward, lit_vertex_colors_backward, sun_project_backward, sun_visibility,
+                        sun_visibility_backward,
                         phong_shade, phong_shade_backward, project_points, shadow_visibility,
                         shadow_visibility_backward,
                         point_lit_vertex_colors, point_lit_vertex_colors_backward, sh_lit_vertex_colors,
@@ -448,7 +453,8 @@ class PhongShadeFunc(torch.autograd.Function):
     def forward(ctx: Any, channels: torch.Tensor, light_directional: Optional[torch.Tensor],  # type: ignore
                 light_ambient, specular, shininess, camera: CameraParams, background,
                 sh: Optional[torch.Tensor] = None, albedo: Optional[torch.Tensor] = None,
-                point_lights: Optional[torch.Tensor] = None, visibility: Optional[torch.Tensor] = None):
+                point_lights: Optional[torch.Tensor] = None, visibility: Optional[torch.Tensor] = None,
+                sun_visibility: Optional[torch.Tensor] = None):
         dev = channels.device
         scalars = [x if isinstance(x, torch.Tensor) else torch.tensor(float(x), dtype=torch.float64, device=dev)
                    for x in (light_ambient, specular, shininess)]
@@ -468,9 +474,12 @@ class PhongShadeFunc(torch.autograd.Function):
         alb = albedo.detach().to(torch.float32).contiguous() if albedo is not None else None
         pl = _f64(point_lights) if point_lights is not None else None
         vis = visibility.detach().to(torch.float32).contiguous() if visibility is not None else None
-        image = phong_shade(ch, params, center, bg, sh=shd, albedo=alb, point_lights=pl, visibility=vis)
-        ctx.save_for_backward(ch, params, center, bg.to(dev, torch.float32), shd, alb, pl, vis)
+        sun = sun_visibility.detach().to(torch.float32).contiguous() if sun_visibility is not None else None
+        image = phong_shade(ch, params, center, bg, sh=shd, albedo=alb, point_lights=pl, visibility=vis,
+                            sun_visibility=sun)
+        ctx.save_for_backward(ch, params, center, bg.to(dev, torch.float32), shd, alb, pl, vis, sun)
         ctx.vis_dtype = visibility.dtype if visibility is not None else None
+        ctx.sun_dtype = sun_visibility.dtype if sun_visibility is not None else None
         ctx.lights_dtype = point_lights.dtype if point_lights is not None else None
         ctx.albedo_dtype = albedo.dtype if albedo is not None else None
         ctx.sh_dtype = sh.dtype if sh is not None else None
@@ -481,11 +490,14 @@ class PhongShadeFunc(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx: Any, image_b: torch.Tensor):  # type: ignore
-        ch, params, center, bg, shd, alb, pl, vis = ctx.saved_tensors
+        ch, params, center, bg, shd, alb, pl, vis, sun = ctx.saved_tensors
         needs = ctx.needs_input_grad
         center_grad = ctx.center_is_input and needs[5]
         shaded = phong_shade_backward(ch, params, center, bg, image_b, _scratch_of(ch.device), center_grad=center_grad,
-                                      sh=shd, albedo=alb, point_lights=pl, visibility=vis)
+                                      sh=shd, albedo=alb, point_lights=pl, visibility=vis, sun_visibility=sun)
+        sun_b = None
+        if sun is not None:
+            shaded, sun_b = shaded[:-1], shaded[-1]
         vis_b = None
         if vis is not None:
             shaded, vis_b = shaded[:-1], shaded[-1]
@@ -507,62 +519,80 @@ class PhongShadeFunc(torch.autograd.Function):
         out.append(albedo_b.to(ctx.albedo_dtype) if albedo_b is not None and needs[8] else None)
         out.append(lights_b.to(ctx.lights_dtype) if lights_b is not None and needs[9] else None)
         out.append(vis_b.to(ctx.vis_dtype) if vis_b is not None and needs[10] else None)
+        out.append(sun_b.to(ctx.sun_dtype) if sun_b is not None and needs[11] else None)
         return tuple(out)
 
 
 class RenderShadowedPhongFunc(torch.autograd.Function):
     """The rasters of a Phong render with shadows, as one node: the G-buffer (beside the albedo raster of a textured
-    mesh, as ``RenderMeshPhongTexturedFunc``) and the 6L cube shadow maps of the point lights (``ShadowCubes``, the
-    model in include/deodr_b200.h), rendered by one ``render_views`` call and back-propagated by one
-    ``render_b_views`` call, the renderer keeping one live forward per slot.  (ij, uv | None, texture | None, channels,
-    depths, edgeflags, vertices [V,3], point_lights [L, 3 + S], albedo scene | None, G-buffer scene, cubes, sigma) ->
-    ([albedo [H,W,C],] G-buffer, maps [6L,M,M]) fp32.  The cube projection happens inside the node, so the maps'
-    gradient reaches the vertices and the lights' positions through its adjoint.  Same snapshot / replay rule as
-    ``RenderMesh2DFunc``."""
+    mesh, as ``RenderMeshPhongTexturedFunc``), the 6L cube shadow maps of the point lights (``ShadowCubes``) and the
+    directional light's map (``SunShadowMap``; the models in include/deodr_b200.h), rendered by one ``render_views``
+    call and back-propagated by one ``render_b_views`` call, the renderer keeping one live forward per slot.  (ij,
+    uv | None, texture | None, channels, depths, edgeflags, vertices [V,3], point_lights [L, 3 + S] | None, albedo
+    scene | None, G-buffer scene, cubes | None, sigma, light_directional [3] | None, sun | None) -> ([albedo [H,W,C],]
+    G-buffer[, maps [6L,M,M]][, sun map [M,M]]) fp32.  The maps' projections happen inside the node, so their gradient
+    reaches the vertices, the lights' positions and the directional light through their adjoints.  Same snapshot /
+    replay rule as ``RenderMesh2DFunc``."""
 
     NAMES = ("ij", "uv", "shade", "texture")
 
     @staticmethod
     def forward(ctx: Any, ij: torch.Tensor, uv: Optional[torch.Tensor], texture: Optional[torch.Tensor],  # type: ignore
                 channels: torch.Tensor, depths: torch.Tensor, edgeflags: torch.Tensor, vertices: torch.Tensor,
-                point_lights: torch.Tensor, albedo_scene: Optional[DeviceScene], gbuffer_scene: DeviceScene,
-                cubes: ShadowCubes, sigma: float = 1.0):
+                point_lights: Optional[torch.Tensor], albedo_scene: Optional[DeviceScene], gbuffer_scene: DeviceScene,
+                cubes: Optional[ShadowCubes], sigma: float = 1.0, light_directional: Optional[torch.Tensor] = None,
+                sun: Optional[SunShadowMap] = None):
         textured = albedo_scene is not None
         if textured:
             check_scene_inputs(albedo_scene, uv=uv, texture=texture)
         check_scene_inputs(gbuffer_scene, colors=channels)
+        if (cubes is None) != (point_lights is None) or (sun is None) != (light_directional is None):
+            raise ValueError("the cube maps come with point_lights, and the sun map with light_directional")
         inputs = (ij.detach(), uv.detach() if textured else None, texture.detach() if textured else None,
-                  channels.detach(), depths.detach(), edgeflags, _f64(vertices.detach()), _f64(point_lights.detach()))
+                  channels.detach(), depths.detach(), edgeflags, _f64(vertices.detach()),
+                  _f64(point_lights.detach()) if cubes is not None else None,
+                  _f64(light_directional.detach()).reshape(3).contiguous() if sun is not None else None)
         ctx.scenes = ([albedo_scene] if textured else []) + [gbuffer_scene]
-        ctx.cubes, ctx.sigma, ctx.textured = cubes, float(sigma), textured
+        ctx.maps = [m for m in (cubes, sun) if m is not None]
+        ctx.cubes, ctx.sun, ctx.sigma, ctx.textured = cubes, sun, float(sigma), textured
         renderer = default_renderer(gbuffer_scene.device.index)
         ctx.fwds = RenderShadowedPhongFunc._render(renderer, ctx, inputs, None)
         ctx.in_dtypes = (ij.dtype, uv.dtype if textured else None, texture.dtype if textured else None, channels.dtype,
-                         vertices.dtype, point_lights.dtype)
+                         vertices.dtype, point_lights.dtype if cubes is not None else None,
+                         light_directional.dtype if sun is not None else None)
         ctx.save_for_backward(*(t.clone() if t is not None else None for t in inputs))
         rasters = tuple(f["image"].clone() for f in ctx.fwds[:len(ctx.scenes)])
-        return rasters + (cubes.maps.clone(),)
+        return rasters + ((cubes.maps.clone(),) if cubes is not None else ()) + \
+            ((sun.map.clone(),) if sun is not None else ())
+
+    @staticmethod
+    def _prepare(ctx, inputs):
+        if ctx.cubes is not None:
+            ctx.cubes.prepare(inputs[6], inputs[7])
+        if ctx.sun is not None:
+            ctx.sun.prepare(inputs[6], inputs[8])
 
     @staticmethod
     def _render(renderer, ctx, inputs, out):
-        ij, uv, texture, channels, depths, edgeflags, vertices, lights = inputs
+        ij, uv, texture, channels, depths, edgeflags = inputs[:6]
         if ctx.textured:
             ctx.scenes[0].update(ij=ij, uv=uv, texture=texture, depths=depths, edgeflags=edgeflags)
         ctx.scenes[-1].update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
-        ctx.cubes.prepare(vertices, lights)
+        RenderShadowedPhongFunc._prepare(ctx, inputs)
         if out is None:
-            out = [renderer._new_outputs(sc, False, False, False) for sc in ctx.scenes] + ctx.cubes.outputs()
-        return renderer.render_views(ctx.scenes + ctx.cubes.scenes, ctx.sigma, out=out)
+            out = [renderer._new_outputs(sc, False, False, False) for sc in ctx.scenes] + \
+                [o for m in ctx.maps for o in m.outputs()]
+        return renderer.render_views(ctx.scenes + [sc for m in ctx.maps for sc in m.scenes], ctx.sigma, out=out)
 
     @staticmethod
     def backward(ctx: Any, *grads):  # type: ignore
         needs = ctx.needs_input_grad
-        if not any(needs[:8]):
-            return (None,) * 12
+        if not any(needs[:8]) and not needs[12]:
+            return (None,) * 14
         inputs = ctx.saved_tensors
         renderer = default_renderer(ctx.scenes[-1].device.index)
         n = len(ctx.scenes)
-        # the shared scenes and cubes may hold another node's inputs by now
+        # the shared scenes and maps may hold another node's inputs by now
         if any(f["generation"] != renderer.generation(f["slot"]) for f in ctx.fwds):
             ctx.fwds = RenderShadowedPhongFunc._render(renderer, ctx, inputs, ctx.fwds)
         else:
@@ -570,27 +600,38 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
                 ctx.scenes[0].update(ij=inputs[0], uv=inputs[1], texture=inputs[2], depths=inputs[4],
                                      edgeflags=inputs[5])
             ctx.scenes[-1].update(ij=inputs[0], colors=inputs[3], depths=inputs[4], edgeflags=inputs[5])
-            ctx.cubes.prepare(inputs[6], inputs[7])
+            RenderShadowedPhongFunc._prepare(ctx, inputs)
         if ctx.textured:
             gs = [requested_grads(ctx.scenes[0], RenderShadowedPhongFunc.NAMES, (True, needs[1], False, needs[2])),
                   ctx.scenes[1].zero_grads()]
         else:
             gs = [ctx.scenes[0].zero_grads()]
         image_bs = [g.to(torch.float32).contiguous() for g in grads[:n]]
-        maps_b = grads[n].to(torch.float32).contiguous()
-        renderer.render_b_views(ctx.scenes + ctx.cubes.scenes, ctx.sigma, ctx.fwds,
-                                image_bs + ctx.cubes.image_bs(maps_b), grads=gs + ctx.cubes.grads())
-        vertices_b, lights_b = cube_project_backward(inputs[6], inputs[7], ctx.cubes.M, ctx.cubes.cameras,
-                                                     ctx.cubes.ij_b, ctx.cubes.colors_b.view(6 * ctx.cubes.L, -1),
-                                                     _scratch_of(inputs[6].device))
-        ij_d, uv_d, tex_d, ch_d, v_d, l_d = ctx.in_dtypes
+        maps_bs = [g.to(torch.float32).contiguous() for g in grads[n:]]
+        if ctx.sun is not None:
+            maps_bs[-1] = maps_bs[-1][None]
+        renderer.render_b_views(ctx.scenes + [sc for m in ctx.maps for sc in m.scenes], ctx.sigma, ctx.fwds,
+                                image_bs + [b for m, mb in zip(ctx.maps, maps_bs) for b in m.image_bs(mb)],
+                                grads=gs + [g for m in ctx.maps for g in m.grads()])
+        scratch = _scratch_of(inputs[6].device)
+        vertices_b = torch.zeros_like(inputs[6])
+        lights_b = light_b = None
+        if ctx.cubes is not None:
+            _, lights_b = cube_project_backward(inputs[6], inputs[7], ctx.cubes.M, ctx.cubes.cameras, ctx.cubes.ij_b,
+                                                ctx.cubes.colors_b.view(6 * ctx.cubes.L, -1), scratch,
+                                                vertices_b=vertices_b)
+        if ctx.sun is not None:
+            _, light_b = sun_project_backward(inputs[6], inputs[8], ctx.sun.bounds, ctx.sun.M, ctx.sun.ij_b[0],
+                                              ctx.sun.colors_b.view(-1), scratch, vertices_b=vertices_b)
+        ij_d, uv_d, tex_d, ch_d, v_d, l_d, d_d = ctx.in_dtypes
         ij_b = sum(g["ij_b"] for g in gs)
         return (ij_b.to(ij_d) if needs[0] else None,
                 gs[0]["uv_b"].to(uv_d) if ctx.textured and needs[1] else None,
                 gs[0]["texture_b"].to(tex_d) if ctx.textured and needs[2] else None,
                 gs[-1]["colors_b"].to(ch_d) if needs[3] else None, None, None,
-                vertices_b.to(v_d) if needs[6] else None, lights_b.to(l_d) if needs[7] else None,
-                None, None, None, None)
+                vertices_b.to(v_d) if needs[6] else None,
+                lights_b.to(l_d) if lights_b is not None and needs[7] else None,
+                None, None, None, None, light_b.to(d_d) if light_b is not None and needs[12] else None, None)
 
 
 class ShadowVisibilityFunc(torch.autograd.Function):
@@ -623,6 +664,37 @@ class ShadowVisibilityFunc(torch.autograd.Function):
                 maps_b.to(md) if needs[2] else None, None, None, None)
 
 
+class SunVisibilityFunc(torch.autograd.Function):
+    """The directional light's visibility of a G-buffer's pixels (deodr_b200_sun_visibility / _b, the model in
+    include/deodr_b200.h): (channels [H,W,C+7], or [H,W,7] beside an albedo, light_directional [3], map [M,M],
+    bounds (cx, cy, cz, r), bias, softness, albedo | None) -> visibility [H,W] fp32.  Backward returns the gradients
+    of the G-buffer's position and coverage slices, of the map and of the light; the albedo, only read for its channel
+    count, gets none."""
+
+    @staticmethod
+    def forward(ctx: Any, channels: torch.Tensor, light_directional: torch.Tensor, sun_map: torch.Tensor,  # type: ignore
+                bounds, bias: float, softness: float, albedo: Optional[torch.Tensor] = None):
+        ch = channels.detach().to(torch.float32).contiguous()
+        ld = _f64(light_directional.detach()).reshape(3).contiguous()
+        mp = sun_map.detach().to(torch.float32).contiguous()
+        alb = albedo.detach() if albedo is not None else None
+        vis = sun_visibility(ch, ld, mp, bounds, bias, softness, albedo=alb)
+        ctx.save_for_backward(ch, ld, mp, alb)
+        ctx.args = (tuple(bounds), float(bias), float(softness))
+        ctx.dtypes = (channels.dtype, light_directional.dtype, sun_map.dtype)
+        return vis
+
+    @staticmethod
+    def backward(ctx: Any, vis_b: torch.Tensor):  # type: ignore
+        ch, ld, mp, alb = ctx.saved_tensors
+        channels_b, map_b, light_b = sun_visibility_backward(ch, ld, mp, *ctx.args, vis_b, _scratch_of(ch.device),
+                                                             albedo=alb)
+        needs = ctx.needs_input_grad
+        cd, ld_d, md = ctx.dtypes
+        return (channels_b.to(cd) if needs[0] else None, light_b.to(ld_d) if needs[1] else None,
+                map_b.to(md) if needs[2] else None, None, None, None, None)
+
+
 project_points_autograd = ProjectPointsFunc.apply
 vertex_normals_autograd = VertexNormalsFunc.apply
 lit_vertex_colors_autograd = LitVertexColorsFunc.apply
@@ -637,6 +709,7 @@ loop_subdivision_autograd = LoopSubdivisionFunc.apply
 phong_shade_autograd = PhongShadeFunc.apply
 render_shadowed_phong = RenderShadowedPhongFunc.apply
 shadow_visibility_autograd = ShadowVisibilityFunc.apply
+sun_visibility_autograd = SunVisibilityFunc.apply
 
 
 def vertex_luminosity_autograd(normals: torch.Tensor, light_directional: Optional[torch.Tensor],
@@ -816,7 +889,10 @@ class Scene3DPytorch:
     light whose position the caller computes from the camera's tensors: its gradient then reaches the camera.  In a
     Phong or textured Phong render, ``set_point_lights(..., shadow_map_size=M)`` makes them cast shadows (the model in
     include/deodr_b200.h): the rasters and the lights' cube maps are one :class:`RenderShadowedPhongFunc` node, the
-    visibility a :class:`ShadowVisibilityFunc`, and the shadows' gradient reaches the vertices and the lights."""
+    visibility a :class:`ShadowVisibilityFunc`, and the shadows' gradient reaches the vertices and the lights.
+    ``set_light(..., shadow_map_size=M, shadow_bias=, shadow_softness=, shadow_bounds=(cx, cy, cz, r))`` makes the
+    directional light cast shadows too: its map is rendered in the same :class:`RenderShadowedPhongFunc` node, its
+    visibility is a :class:`SunVisibilityFunc`, and a light that requires grad receives the shadow's share."""
 
     def __init__(self, sigma: float = 1.0, backface_culling: bool = True, shading: str = "gouraud"):
         if shading not in ("gouraud", "phong", "phong_textured"):
@@ -831,6 +907,9 @@ class Scene3DPytorch:
         self.point_lights: Optional[torch.Tensor] = None
         self.shadow_map_size, self.shadow_bias, self.shadow_softness = 0, None, None
         self._cubes: Dict[tuple, ShadowCubes] = {}
+        self.light_shadow_map_size, self.light_shadow_bias, self.light_shadow_softness = 0, None, None
+        self.light_shadow_bounds: Optional[tuple] = None
+        self._suns: Dict[tuple, SunShadowMap] = {}
         self.specular: Any = 0.0
         self.shininess: Any = 16.0
         self.background_color: Optional[np.ndarray] = None
@@ -841,6 +920,7 @@ class Scene3DPytorch:
     def set_mesh(self, mesh: ColoredTriMeshPytorch) -> None:
         self.mesh = mesh
         self._cubes = {}
+        self._suns = {}
         self._scenes = {}
         self._phong_scenes = {}
         self._albedo_scenes = {}
@@ -853,9 +933,19 @@ class Scene3DPytorch:
                                          torch.tensor(float(x), dtype=torch.float64, device=dev)
                                          for x in (specular, shininess)]
 
-    def set_light(self, light_directional, light_ambient) -> None:
+    def set_light(self, light_directional, light_ambient, shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
+                  shadow_softness: Optional[float] = None, shadow_bounds=None) -> None:
         """``light_directional`` [3] (None: ambient light only) and ``light_ambient`` (a number or 0-d tensor); tensors
-        are used as given, so a light that requires grad receives its gradient."""
+        are used as given, so a light that requires grad receives its gradient.  A ``shadow_map_size`` M > 0 makes
+        the directional light cast shadows in a Phong render (the model in include/deodr_b200.h), with
+        ``shadow_bias``, ``shadow_softness`` and ``shadow_bounds`` = (cx, cy, cz, r) (world units, all required) and
+        the refusals of ``DeviceMeshView``'s ``light_shadow_*`` arguments."""
+        size = check_sun_shadow_arguments(self.shading, light_directional, shadow_map_size, shadow_bias,
+                                          shadow_softness, shadow_bounds)
+        self.light_shadow_map_size = size
+        self.light_shadow_bias = float(shadow_bias) if size else None
+        self.light_shadow_softness = float(shadow_softness) if size else None
+        self.light_shadow_bounds = tuple(float(b) for b in shadow_bounds) if size else None
         dev = self.mesh.device if self.mesh is not None else _device(None)
         if light_directional is not None and not isinstance(light_directional, torch.Tensor):
             light_directional = torch.as_tensor(np.asarray(light_directional, dtype=np.float64), device=dev)
@@ -982,21 +1072,19 @@ class Scene3DPytorch:
         ij, depths = camera.project_points(m.vertices)
         ones = torch.ones((m.nb_vertices, 1), dtype=torch.float64, device=m.device)
         channels = torch.cat((m.vertex_normals, m.vertices.to(torch.float64), ones), dim=1)
-        vis = None
-        if self.shadow_map_size:
-            albedo, gbuffer, maps = render_shadowed_phong(ij, uv, texture, channels, depths, self._edgeflags(ij),
-                                                          m.vertices, self.point_lights,
-                                                          self._albedo_scene(camera, uv, texture),
-                                                          self._phong_scene(camera, 0), self._shadow_cubes(), self.sigma)
-            vis = shadow_visibility_autograd(gbuffer, self.point_lights, maps, self.shadow_bias, self.shadow_softness,
-                                             albedo)
+        vis = sun = None
+        if self.shadow_map_size or self.light_shadow_map_size:
+            out = self._render_shadowed(ij, uv, texture, channels, depths, self._albedo_scene(camera, uv, texture),
+                                        self._phong_scene(camera, 0))
+            albedo, gbuffer = out[:2]
+            vis, sun = self._visibilities(gbuffer, out[2:], albedo)
         else:
             albedo, gbuffer = render_mesh_phong_textured(ij, uv, texture, channels, depths, self._edgeflags(ij),
                                                          self._albedo_scene(camera, uv, texture),
                                                          self._phong_scene(camera, 0), self.sigma)
         return phong_shade_autograd(gbuffer, self.light_directional, self.light_ambient, self.specular,
                                     self.shininess, camera.center() if camera.is_tensor else camera,
-                                    self.background_color, self.light_sh, albedo, self.point_lights, vis)
+                                    self.background_color, self.light_sh, albedo, self.point_lights, vis, sun)
 
     def _render_phong(self, camera: CameraPytorch) -> torch.Tensor:
         m = self.mesh
@@ -1012,18 +1100,46 @@ class Scene3DPytorch:
         ones = torch.ones((m.nb_vertices, 1), dtype=torch.float64, device=m.device)
         channels = torch.cat((m.vertices_colors.to(torch.float64), m.vertex_normals, m.vertices.to(torch.float64),
                               ones), dim=1)
-        vis = None
-        if self.shadow_map_size:
-            raster, maps = render_shadowed_phong(ij, None, None, channels, depths, self._edgeflags(ij), m.vertices,
-                                                 self.point_lights, None, self._phong_scene(camera, nc),
-                                                 self._shadow_cubes(), self.sigma)
-            vis = shadow_visibility_autograd(raster, self.point_lights, maps, self.shadow_bias, self.shadow_softness)
+        vis = sun = None
+        if self.shadow_map_size or self.light_shadow_map_size:
+            out = self._render_shadowed(ij, None, None, channels, depths, None, self._phong_scene(camera, nc))
+            raster = out[0]
+            vis, sun = self._visibilities(raster, out[1:], None)
         else:
             raster = render_mesh_2d(ij, channels, depths, self._edgeflags(ij), self._phong_scene(camera, nc),
                                     self.sigma)
         return phong_shade_autograd(raster, self.light_directional, self.light_ambient, self.specular, self.shininess,
                                     camera.center() if camera.is_tensor else camera, self.background_color,
-                                    self.light_sh, None, self.point_lights, vis)
+                                    self.light_sh, None, self.point_lights, vis, sun)
+
+    def _render_shadowed(self, ij, uv, texture, channels, depths, albedo_scene, gbuffer_scene) -> tuple:
+        """The rasters and the shadow maps in one :class:`RenderShadowedPhongFunc` node."""
+        m = self.mesh
+        cubes = self._shadow_cubes() if self.shadow_map_size else None
+        sun = self._sun_map() if self.light_shadow_map_size else None
+        return render_shadowed_phong(ij, uv, texture, channels, depths, self._edgeflags(ij), m.vertices,
+                                     self.point_lights if cubes is not None else None, albedo_scene, gbuffer_scene,
+                                     cubes, self.sigma, self.light_directional if sun is not None else None, sun)
+
+    def _visibilities(self, gbuffer, maps, albedo) -> tuple:
+        """(the point lights' visibility or None, the directional light's or None) from the node's maps."""
+        vis = sun = None
+        if self.shadow_map_size:
+            vis = shadow_visibility_autograd(gbuffer, self.point_lights, maps[0], self.shadow_bias,
+                                             self.shadow_softness, albedo)
+        if self.light_shadow_map_size:
+            sun = sun_visibility_autograd(gbuffer, self.light_directional, maps[-1], self.light_shadow_bounds,
+                                          self.light_shadow_bias, self.light_shadow_softness, albedo)
+        return vis, sun
+
+    def _sun_map(self) -> SunShadowMap:
+        """The cached directional-light shadow map of the mesh for the map size and the window."""
+        m = self.mesh
+        key = (self.light_shadow_map_size, self.light_shadow_bounds)
+        if key not in self._suns:
+            self._suns[key] = SunShadowMap(np.ascontiguousarray(m.faces, dtype=np.uint32), m.nb_vertices, key[0],
+                                           key[1], m.clockwise, m.device)
+        return self._suns[key]
 
     def _shadow_cubes(self) -> ShadowCubes:
         """The cached cube shadow maps of the mesh for the lights' count and the map size."""

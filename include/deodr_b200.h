@@ -736,6 +736,79 @@ int deodr_b200_point_phong_shade_shadowed_b(const DeodrPhongIO *io, const float 
                                             int nb_lights, int light_channels, double *lights_b, const float *vis,
                                             float *vis_b, double *scratch, void *stream);
 
+/* ---- shadows from the directional light --------------------------------------------------------------------------
+ * The directional light l = params[0..2] of DeodrPhongIO (in device memory) gets one orthographic shadow map of M x M
+ * texels (M from 8 to 4096) over a window the caller fixes: a centre c (3) and a radius r > 0 in world units, host
+ * values (the light has no position, so no default is free of scale).  With d = l / |l| the direction the light
+ * travels (d = +z where |l| = 0, so that the map stays finite), the frame is Frisvad's orthonormal basis around d:
+ *
+ *   d_z < -0.9999999:  e1 = (0, -1, 0),  e2 = (-1, 0, 0)
+ *   otherwise:         a = 1 / (1 + d_z),  b = -d_x d_y a,  e1 = (1 - d_x^2 a, b, -d_x),  e2 = (b, 1 - d_y^2 a, -d_y)
+ *
+ * (e1, e2, d) is a proper rotation, so the map keeps the mesh's winding.  The frame is smooth except at the pole
+ * d = -z, where the map's rotation about d (never d itself) jumps: a camera looking along +z with the light beside it
+ * puts the pole behind the scene.  Inside the pole's band the fixed e1 and e2 are orthogonal to d only to within
+ * |d_xy| < 4.5e-4 (Frisvad's construction).  A point x projects to
+ *
+ *   u = (M-1)/2 + phi <e1, x - c> / r,   v = (M-1)/2 + phi <e2, x - c> / r,   z = <d, x - c> + 2 r,   phi = M/2 - 2
+ *
+ * so that a point of the sphere |x - c| <= r has its 2x2 taps inside the map and z in [r, 3r].  The map D [M,M] is
+ * the depth render of (u, v, z) (the recipe of the cube faces above: the vertex depth as a one-channel colour, the
+ * caller's sigma in map pixels, the mesh's winding, culling on, a background of DEODR_B200_SHADOW_FAR).  The
+ * visibility of x (per pixel x = X / a) is the cube maps' soft test on (u, v, z) - the 2x2 lerp of
+ * s((D + bias - z) / softness + 1) - and V = 1 exactly, with zero gradient, where a = 0, where x is not finite, where
+ * |x - c| > r (receivers outside the window are lit: a limitation) or where |l| = 0.  Shading: per pixel the
+ * directional diff and spec are each multiplied by V, each product rounded on its own, so that where V = 1 the image
+ * is bit for bit the image without the sun's shadow; every other term (ambient, environment, point lights and their
+ * own V_j) is unchanged.
+ *
+ * Adjoint: from sun_vis_b [H,W] = sum_c image_b[c] (A[c] diff + spec), the gradient goes to x (the G-buffer's
+ * position slice and, through x = X / a, its coverage slice), to the map's texels (fp32 atomics) and to l through
+ * (e1, e2, d); the map's gradient then goes through the rasteriser's adjoint of the one depth render, whose ij_b and
+ * depths_b the projection's adjoint takes to the vertices and to l.  l receives (I - d d^T) / |l| applied to the
+ * gradient of d: the intensity |l| gets nothing from the shadow.  Every fp64 sum is taken in a fixed order, without
+ * fp64 atomics.  The limitations of the cube maps on triangle size and open surfaces apply too. */
+
+/* The projection of vertices [n,3] into the sun map: ij [n,2] and depths [n] fp64, written; light [3] fp64 device
+ * (read on the device, nothing read back), center [3] host.  DEODR_B200_EINVAL before any launch for n < 1, a NULL
+ * buffer, map_size outside [8, 4096], a non-finite center or a non-finite or non-positive radius.  No host
+ * synchronisation. */
+int deodr_b200_sun_project(const double *vertices, int n, const double *light, const double *center, double radius,
+                           int map_size, double *ij, double *depths, void *stream);
+/* Its adjoint from ij_b [n,2] and depths_b [n] (fp32, the rasteriser's): vertices_b [n,3] accumulated, one thread per
+ * vertex (no atomics), and light_b [3] accumulated, summed in a fixed order (`scratch` of
+ * deodr_b200_fitter_scratch_bytes).  Same refusals, plus a NULL vertices_b, light_b or scratch. */
+int deodr_b200_sun_project_b(const double *vertices, int n, const double *light, const double *center, double radius,
+                             int map_size, const float *ij_b, const float *depths_b, double *vertices_b,
+                             double *light_b, double *scratch, void *stream);
+/* The visibility sun_vis [H,W] fp32 of the G-buffer's pixels (io's channels, params, H, W, C, off_position and
+ * off_coverage as for deodr_b200_shadow_visibility) under the sun map map [M,M] fp32.  DEODR_B200_EINVAL before any
+ * launch for a NULL buffer, bad io sizes or offsets, map_size outside [8, 4096], a non-finite or non-positive bias,
+ * softness or radius, or a non-finite center.  No host synchronisation. */
+int deodr_b200_sun_visibility(const DeodrPhongIO *io, const double *center, double radius, const float *map,
+                              int map_size, double bias, double softness, float *vis, void *stream);
+/* Its adjoint from vis_b [H,W] fp32: io->channels_b's position and coverage slices accumulated, map_b [M,M]
+ * accumulated with fp32 atomics, and light_b [3] (l's gradient; params_b of the shading's adjoint may be passed)
+ * accumulated, summed in a fixed order.  Same refusals, plus a NULL channels_b, vis_b, map_b, light_b or scratch. */
+int deodr_b200_sun_visibility_b(const DeodrPhongIO *io, const double *center, double radius, const float *map,
+                                int map_size, double bias, double softness, const float *vis_b, float *map_b,
+                                double *light_b, double *scratch, void *stream);
+/* The Phong shading (either form: albedo NULL reads it from the G-buffer) with the directional terms multiplied by
+ * sun_vis [H,W] fp32, with an optional environment (sh NULL with sh_channels 0), and optional point lights (lights
+ * NULL with nb_lights 0) with their optional visibility vis [H,W,L].  The refusals of the calls it extends, plus a
+ * NULL sun_vis; DEODR_B200_EUNSUPPORTED for bad channel or light counts. */
+int deodr_b200_phong_shade_sun_shadowed(const DeodrPhongIO *io, const float *albedo, const double *sh,
+                                        int sh_channels, const double *lights, int nb_lights, int light_channels,
+                                        const float *vis, const float *sun_vis, void *stream);
+/* Its adjoint, which also writes sun_vis_b [H,W] fp32 = sum_c image_b[c] (A[c] diff + spec), and, with point lights,
+ * lights_b (and, with vis, vis_b as deodr_b200_point_phong_shade_shadowed_b).  Its refusals, plus a NULL sun_vis or
+ * sun_vis_b. */
+int deodr_b200_phong_shade_sun_shadowed_b(const DeodrPhongIO *io, const float *albedo, float *albedo_b,
+                                          const double *sh, int sh_channels, double *sh_b, const double *lights,
+                                          int nb_lights, int light_channels, double *lights_b, const float *vis,
+                                          float *vis_b, const float *sun_vis, float *sun_vis_b, double *scratch,
+                                          void *stream);
+
 /* One parameter vector of a heavy-ball update (device pointers, `size` entries each):
  *   step = clamp(-grad * factor, -max_step, max_step)   (max_step = INFINITY: unclamped)
  *   speed = (1 - damping) (speed * inertia + (1 - inertia) step);  value += speed
