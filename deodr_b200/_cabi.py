@@ -379,6 +379,14 @@ SYMBOLS = [
     ("deodr_b200_phong_shade_sun_shadowed_b", C.c_int,
      [C.POINTER(PhongIO), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_vertex_tangents", C.c_int,
+     [C.POINTER(MeshTopology), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_vertex_tangents_b", C.c_int,
+     [C.POINTER(MeshTopology), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_normal_map", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_normal_map_b", C.c_int,
+     [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("deodr_b200_fitter_update", C.c_int,
      [C.POINTER(HeavyBall), C.c_void_p, C.POINTER(HeavyBall), C.c_int, C.c_double, C.c_double, C.c_void_p,
       C.c_void_p, C.c_void_p, C.c_void_p]),

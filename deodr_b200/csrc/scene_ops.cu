@@ -858,6 +858,270 @@ __global__ void k_face_normals_b(DeodrMeshTopology m, const double *vertices, co
     }
 }
 
+// ---- tangent frames and normal maps (the model in include/deodr_b200.h) --------------------------------------------
+
+struct FaceTangent {
+    double e1[3], e2[3], du1, dv1, du2, dv2, sigma;
+};
+
+// face f's edges, uv deltas and sigma = sign(det); t_f = sigma (dv2 e1 - dv1 e2), b_f = sigma (du1 e2 - du2 e1)
+__device__ __forceinline__ FaceTangent face_tangent(const DeodrMeshTopology &m, const double *vertices,
+                                                    const uint32_t *faces_uv, const double *uv, int f, double t[3],
+                                                    double b[3]) {
+    FaceTangent q;
+    const uint32_t i0 = m.faces[3 * (size_t)f], i1 = m.faces[3 * (size_t)f + 1], i2 = m.faces[3 * (size_t)f + 2];
+    const uint32_t k0 = faces_uv[3 * (size_t)f], k1 = faces_uv[3 * (size_t)f + 1], k2 = faces_uv[3 * (size_t)f + 2];
+    for (int j = 0; j < 3; j++) {
+        q.e1[j] = vertices[3 * (size_t)i1 + j] - vertices[3 * (size_t)i0 + j];
+        q.e2[j] = vertices[3 * (size_t)i2 + j] - vertices[3 * (size_t)i0 + j];
+    }
+    q.du1 = uv[2 * (size_t)k1] - uv[2 * (size_t)k0];
+    q.dv1 = uv[2 * (size_t)k1 + 1] - uv[2 * (size_t)k0 + 1];
+    q.du2 = uv[2 * (size_t)k2] - uv[2 * (size_t)k0];
+    q.dv2 = uv[2 * (size_t)k2 + 1] - uv[2 * (size_t)k0 + 1];
+    const double det = q.du1 * q.dv2 - q.du2 * q.dv1;
+    q.sigma = det > 0 ? 1.0 : (det < 0 ? -1.0 : 0.0);
+    for (int j = 0; j < 3; j++) {
+        t[j] = q.sigma * (q.dv2 * q.e1[j] - q.dv1 * q.e2[j]);
+        b[j] = q.sigma * (q.du1 * q.e2[j] - q.du2 * q.e1[j]);
+    }
+    return q;
+}
+
+// x / |x|, or 0 when |x| = 0
+__device__ __forceinline__ void unit_or_zero(const double x[3], double out[3]) {
+    const double norm = sqrt((x[0] * x[0] + x[1] * x[1]) + x[2] * x[2]);
+    for (int j = 0; j < 3; j++) out[j] = norm > 0 ? x[j] / norm : 0.0;
+}
+
+// the adjoint of unit_or_zero: 0 when |x| = 0
+__device__ __forceinline__ void unit_or_zero_b(const double x[3], const double xn_b[3], double out[3]) {
+    const double n2 = (x[0] * x[0] + x[1] * x[1]) + x[2] * x[2];
+    if (!(n2 > 0)) {
+        for (int j = 0; j < 3; j++) out[j] = 0.0;
+        return;
+    }
+    normalize_b(x, xn_b, out);
+}
+
+__global__ void k_face_tangents(DeodrMeshTopology m, const double *vertices, const uint32_t *faces_uv,
+                                const double *uv, double *face_frames) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= m.nb_faces) return;
+    double t[3], b[3];
+    face_tangent(m, vertices, faces_uv, uv, f, t, b);
+    for (int j = 0; j < 3; j++) {
+        face_frames[6 * (size_t)f + j] = t[j];
+        face_frames[6 * (size_t)f + 3 + j] = b[j];
+    }
+}
+
+// T_v, B_v: the face terms summed over the vertex-face CSR in its order (as k_vertex_normals), then normalised
+__global__ void k_vertex_tangents(DeodrMeshTopology m, const double *face_frames, double *frames) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= m.nb_vertices) return;
+    double s[6] = {0, 0, 0, 0, 0, 0};
+    for (int k = m.vertex_face_offset[v]; k < m.vertex_face_offset[v + 1]; k++) {
+        const int f = m.vertex_face_index[k];
+        for (int j = 0; j < 6; j++) s[j] += face_frames[6 * (size_t)f + j];
+    }
+    double out[6];
+    unit_or_zero(s, out);
+    unit_or_zero(s + 3, out + 3);
+    for (int j = 0; j < 6; j++) frames[6 * (size_t)v + j] = out[j];
+}
+
+// per vertex: the sums' adjoint (the sums recomputed from the faces in the forward's order)
+__global__ void k_vertex_tangents_b1(DeodrMeshTopology m, const double *vertices, const uint32_t *faces_uv,
+                                     const double *uv, const double *frames_b, double *sum_b) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= m.nb_vertices) return;
+    double s[6] = {0, 0, 0, 0, 0, 0};
+    for (int k = m.vertex_face_offset[v]; k < m.vertex_face_offset[v + 1]; k++) {
+        double t[3], b[3];
+        face_tangent(m, vertices, faces_uv, uv, m.vertex_face_index[k], t, b);
+        for (int j = 0; j < 3; j++) {
+            s[j] += t[j];
+            s[3 + j] += b[j];
+        }
+    }
+    double g[6], out[6];
+    for (int j = 0; j < 6; j++) g[j] = frames_b[6 * (size_t)v + j];
+    unit_or_zero_b(s, g, out);
+    unit_or_zero_b(s + 3, g + 3, out + 3);
+    for (int j = 0; j < 6; j++) sum_b[6 * (size_t)v + j] = out[j];
+}
+
+// per face: t_f_b and b_f_b gathered from its corners, taken to (e1_b, e2_b, du1_b, dv1_b, du2_b, dv2_b) [10]
+__global__ void k_face_tangents_b(DeodrMeshTopology m, const double *vertices, const uint32_t *faces_uv,
+                                  const double *uv, const double *sum_b, double *face_b) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= m.nb_faces) return;
+    double t[3], b[3], tb[3] = {0, 0, 0}, bb[3] = {0, 0, 0};
+    const FaceTangent q = face_tangent(m, vertices, faces_uv, uv, f, t, b);
+    for (int c = 0; c < 3; c++) {
+        const uint32_t id = m.faces[3 * (size_t)f + c];
+        for (int j = 0; j < 3; j++) {
+            tb[j] += sum_b[6 * (size_t)id + j];
+            bb[j] += sum_b[6 * (size_t)id + 3 + j];
+        }
+    }
+    double *o = face_b + 10 * (size_t)f;
+    for (int j = 0; j < 3; j++) {
+        o[j] = q.sigma * (q.dv2 * tb[j] - q.du2 * bb[j]);
+        o[3 + j] = q.sigma * (q.du1 * bb[j] - q.dv1 * tb[j]);
+    }
+    o[6] = q.sigma * ((q.e2[0] * bb[0] + q.e2[1] * bb[1]) + q.e2[2] * bb[2]);
+    o[7] = -q.sigma * ((q.e2[0] * tb[0] + q.e2[1] * tb[1]) + q.e2[2] * tb[2]);
+    o[8] = -q.sigma * ((q.e1[0] * bb[0] + q.e1[1] * bb[1]) + q.e1[2] * bb[2]);
+    o[9] = q.sigma * ((q.e1[0] * tb[0] + q.e1[1] * tb[1]) + q.e1[2] * tb[2]);
+}
+
+// per position vertex: the corners it holds in its faces (a face listed twice in the CSR, for a repeated corner, is
+// visited once and adds every such corner), accumulated into vertices_b in the CSR's order
+__global__ void k_tangents_vertices_b(DeodrMeshTopology m, const double *face_b, double *vertices_b) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= m.nb_vertices) return;
+    double acc[3] = {0, 0, 0};
+    const int k0 = m.vertex_face_offset[v];
+    for (int k = k0; k < m.vertex_face_offset[v + 1]; k++) {
+        const int f = m.vertex_face_index[k];
+        if (k > k0 && m.vertex_face_index[k - 1] == f) continue;
+        const double *o = face_b + 10 * (size_t)f;
+        for (int c = 0; c < 3; c++) {
+            if (m.faces[3 * (size_t)f + c] != (uint32_t)v) continue;
+            for (int j = 0; j < 3; j++) acc[j] += c == 0 ? -o[j] - o[3 + j] : o[3 * (c - 1) + j];
+        }
+    }
+    for (int j = 0; j < 3; j++) vertices_b[3 * (size_t)v + j] += acc[j];
+}
+
+// per uv vertex, the same gather over the uv-vertex-face CSR into uv_b (overwritten)
+__global__ void k_tangents_uv_b(const uint32_t *faces_uv, const int32_t *uv_face_offset, const int32_t *uv_face_index,
+                                int nb_uv, const double *face_b, double *uv_b) {
+    const int u = blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= nb_uv) return;
+    double acc[2] = {0, 0};
+    const int k0 = uv_face_offset[u];
+    for (int k = k0; k < uv_face_offset[u + 1]; k++) {
+        const int f = uv_face_index[k];
+        if (k > k0 && uv_face_index[k - 1] == f) continue;
+        const double *o = face_b + 10 * (size_t)f;
+        for (int c = 0; c < 3; c++) {
+            if (faces_uv[3 * (size_t)f + c] != (uint32_t)u) continue;
+            if (c == 0) {
+                acc[0] += -(o[6] + o[8]);
+                acc[1] += -(o[7] + o[9]);
+            } else {
+                acc[0] += o[6 + 2 * (c - 1)];
+                acc[1] += o[7 + 2 * (c - 1)];
+            }
+        }
+    }
+    uv_b[2 * (size_t)u] = acc[0];
+    uv_b[2 * (size_t)u + 1] = acc[1];
+}
+
+struct NormalMapFrame {
+    double n[3], tt[3], t[3], bt[3], s, p[3];
+};
+
+// one pixel's frame and perturbed direction p = (M_x t + M_y b) + M_z n from the 13-channel G-buffer (N, X, a, T, B)
+// and the map raster M
+__device__ __forceinline__ NormalMapFrame normal_map_frame(const float *g, const double M[3]) {
+    NormalMapFrame q;
+    const double N[3] = {g[0], g[1], g[2]}, T[3] = {g[7], g[8], g[9]}, B[3] = {g[10], g[11], g[12]};
+    unit_or_zero(N, q.n);
+    const double tn = (T[0] * q.n[0] + T[1] * q.n[1]) + T[2] * q.n[2];
+    for (int j = 0; j < 3; j++) q.tt[j] = T[j] - tn * q.n[j];
+    unit_or_zero(q.tt, q.t);
+    q.bt[0] = q.n[1] * q.t[2] - q.n[2] * q.t[1];
+    q.bt[1] = q.n[2] * q.t[0] - q.n[0] * q.t[2];
+    q.bt[2] = q.n[0] * q.t[1] - q.n[1] * q.t[0];
+    q.s = ((q.bt[0] * B[0] + q.bt[1] * B[1]) + q.bt[2] * B[2]) >= 0 ? 1.0 : -1.0;
+    for (int j = 0; j < 3; j++) q.p[j] = (M[0] * q.t[j] + M[1] * (q.s * q.bt[j])) + M[2] * q.n[j];
+    return q;
+}
+
+__global__ void __launch_bounds__(BLOCK) k_normal_map(const float *gbuffer, const float *map, long long pixels,
+                                                      float *out) {
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= pixels) return;
+    const float *g = gbuffer + 13 * i;
+    float *o = out + 7 * i;
+    for (int j = 3; j < 7; j++) o[j] = g[j];
+    const double a = g[6];
+    double np[3] = {0, 0, 0};
+    if (a != 0) {
+        const double M[3] = {map[3 * i], map[3 * i + 1], map[3 * i + 2]};
+        const NormalMapFrame q = normal_map_frame(g, M);
+        double u[3];
+        unit_or_zero(q.p, u);
+        for (int j = 0; j < 3; j++) np[j] = a * u[j];
+    }
+    for (int j = 0; j < 3; j++) o[j] = (float)np[j];
+}
+
+__global__ void __launch_bounds__(BLOCK) k_normal_map_b(const float *gbuffer, const float *map, long long pixels,
+                                                        const float *out_b, float *gbuffer_b, float *map_b) {
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= pixels) return;
+    const float *g = gbuffer + 13 * i, *ob = out_b + 7 * i;
+    float *gb = gbuffer_b + 13 * i;
+    const double a = g[6];
+    double N_b[3] = {0, 0, 0}, T_b[3] = {0, 0, 0}, M_b[3] = {0, 0, 0}, a_b = ob[6];
+    const double np_b[3] = {ob[0], ob[1], ob[2]};
+    if (a != 0) {
+        const double M[3] = {map[3 * i], map[3 * i + 1], map[3 * i + 2]};
+        const NormalMapFrame q = normal_map_frame(g, M);
+        const double pn2 = (q.p[0] * q.p[0] + q.p[1] * q.p[1]) + q.p[2] * q.p[2];
+        if (pn2 > 0) {
+            double u[3], u_b[3], p_b[3];
+            unit_or_zero(q.p, u);
+            a_b += (np_b[0] * u[0] + np_b[1] * u[1]) + np_b[2] * u[2];
+            for (int j = 0; j < 3; j++) u_b[j] = a * np_b[j];
+            normalize_b(q.p, u_b, p_b);
+            double b[3], t_b[3], bt_b[3], n_b[3];
+            for (int j = 0; j < 3; j++) b[j] = q.s * q.bt[j];
+            M_b[0] = (p_b[0] * q.t[0] + p_b[1] * q.t[1]) + p_b[2] * q.t[2];
+            M_b[1] = (p_b[0] * b[0] + p_b[1] * b[1]) + p_b[2] * b[2];
+            M_b[2] = (p_b[0] * q.n[0] + p_b[1] * q.n[1]) + p_b[2] * q.n[2];
+            for (int j = 0; j < 3; j++) {
+                t_b[j] = M[0] * p_b[j];
+                bt_b[j] = q.s * (M[1] * p_b[j]);
+                n_b[j] = M[2] * p_b[j];
+            }
+            // bt = n x t: n_b += t x bt_b, t_b += bt_b x n
+            n_b[0] += q.t[1] * bt_b[2] - q.t[2] * bt_b[1];
+            n_b[1] += q.t[2] * bt_b[0] - q.t[0] * bt_b[2];
+            n_b[2] += q.t[0] * bt_b[1] - q.t[1] * bt_b[0];
+            t_b[0] += bt_b[1] * q.n[2] - bt_b[2] * q.n[1];
+            t_b[1] += bt_b[2] * q.n[0] - bt_b[0] * q.n[2];
+            t_b[2] += bt_b[0] * q.n[1] - bt_b[1] * q.n[0];
+            // t = tt / |tt|, tt = T - <T, n> n
+            double tt_b[3];
+            unit_or_zero_b(q.tt, t_b, tt_b);
+            const double T[3] = {g[7], g[8], g[9]};
+            const double tn = (T[0] * q.n[0] + T[1] * q.n[1]) + T[2] * q.n[2];
+            const double ntt_b = (q.n[0] * tt_b[0] + q.n[1] * tt_b[1]) + q.n[2] * tt_b[2];
+            for (int j = 0; j < 3; j++) {
+                T_b[j] = tt_b[j] - ntt_b * q.n[j];
+                n_b[j] -= tn * tt_b[j] + ntt_b * T[j];
+            }
+            const double N[3] = {g[0], g[1], g[2]};
+            unit_or_zero_b(N, n_b, N_b);
+        }
+    }
+    for (int j = 0; j < 3; j++) {
+        gb[j] = (float)N_b[j];
+        gb[3 + j] = ob[3 + j];
+        gb[7 + j] = (float)T_b[j];
+        gb[10 + j] = 0.0f;
+        map_b[3 * i + j] = (float)M_b[j];
+    }
+    gb[6] = (float)a_b;
+}
+
 int check_launch() {
     CUDA_TRY(cudaGetLastError());
     return DEODR_B200_OK;
@@ -1137,6 +1401,55 @@ int deodr_b200_sun_visibility_b(const DeodrPhongIO *io, const double *center, do
         io->channels, io->channels_b, pixels, stride, io->off_position, io->off_coverage, io->params,
         sun_window(center, radius, map_size), map, bias, softness, vis_b, map_b, light_b,
         reinterpret_cast<Scratch *>(scratch));
+    return check_launch();
+}
+
+int deodr_b200_vertex_tangents(const DeodrMeshTopology *mesh, const double *vertices, const uint32_t *faces_uv,
+                               const double *uv, int nb_uv, double *face_frames, double *frames, void *stream) {
+    if (!mesh || !mesh->faces || !mesh->vertex_face_offset || !mesh->vertex_face_index || mesh->nb_faces < 1 ||
+        mesh->nb_vertices < 1 || nb_uv < 1 || !vertices || !faces_uv || !uv || !face_frames || !frames)
+        return set_error(DEODR_B200_EINVAL, "vertex_tangents: bad argument (T, V and nb_uv >= 1, every pointer "
+                                            "non-NULL, the vertex-face CSR given)");
+    cudaStream_t st = (cudaStream_t)stream;
+    k_face_tangents<<<grid_of(mesh->nb_faces), BLOCK, 0, st>>>(*mesh, vertices, faces_uv, uv, face_frames);
+    k_vertex_tangents<<<grid_of(mesh->nb_vertices), BLOCK, 0, st>>>(*mesh, face_frames, frames);
+    return check_launch();
+}
+
+int deodr_b200_vertex_tangents_b(const DeodrMeshTopology *mesh, const double *vertices, const uint32_t *faces_uv,
+                                 const double *uv, int nb_uv, const int32_t *uv_face_offset,
+                                 const int32_t *uv_face_index, const double *frames_b, double *scratch,
+                                 double *vertices_b, double *uv_b, void *stream) {
+    if (!mesh || !mesh->faces || !mesh->vertex_face_offset || !mesh->vertex_face_index || mesh->nb_faces < 1 ||
+        mesh->nb_vertices < 1 || nb_uv < 1 || !vertices || !faces_uv || !uv || !uv_face_offset || !uv_face_index ||
+        !frames_b || !scratch || !vertices_b || !uv_b)
+        return set_error(DEODR_B200_EINVAL, "vertex_tangents_b: bad argument (T, V and nb_uv >= 1, every pointer "
+                                            "non-NULL, the vertex-face CSR given)");
+    cudaStream_t st = (cudaStream_t)stream;
+    double *sum_b = scratch, *face_b = scratch + 6 * (size_t)mesh->nb_vertices;
+    k_vertex_tangents_b1<<<grid_of(mesh->nb_vertices), BLOCK, 0, st>>>(*mesh, vertices, faces_uv, uv, frames_b, sum_b);
+    k_face_tangents_b<<<grid_of(mesh->nb_faces), BLOCK, 0, st>>>(*mesh, vertices, faces_uv, uv, sum_b, face_b);
+    k_tangents_vertices_b<<<grid_of(mesh->nb_vertices), BLOCK, 0, st>>>(*mesh, face_b, vertices_b);
+    k_tangents_uv_b<<<grid_of(nb_uv), BLOCK, 0, st>>>(faces_uv, uv_face_offset, uv_face_index, nb_uv, face_b, uv_b);
+    return check_launch();
+}
+
+int deodr_b200_normal_map(const float *gbuffer, const float *map, int H, int W, float *out, void *stream) {
+    if (!gbuffer || !map || !out || H < 1 || W < 1)
+        return set_error(DEODR_B200_EINVAL, "normal_map: bad argument (H, W >= 1, every pointer non-NULL)");
+    const long long pixels = (long long)H * W;
+    k_normal_map<<<(unsigned)((pixels + BLOCK - 1) / BLOCK), BLOCK, 0, (cudaStream_t)stream>>>(gbuffer, map, pixels,
+                                                                                               out);
+    return check_launch();
+}
+
+int deodr_b200_normal_map_b(const float *gbuffer, const float *map, int H, int W, const float *out_b,
+                            float *gbuffer_b, float *map_b, void *stream) {
+    if (!gbuffer || !map || !out_b || !gbuffer_b || !map_b || H < 1 || W < 1)
+        return set_error(DEODR_B200_EINVAL, "normal_map_b: bad argument (H, W >= 1, every pointer non-NULL)");
+    const long long pixels = (long long)H * W;
+    k_normal_map_b<<<(unsigned)((pixels + BLOCK - 1) / BLOCK), BLOCK, 0, (cudaStream_t)stream>>>(
+        gbuffer, map, pixels, out_b, gbuffer_b, map_b);
     return check_launch();
 }
 

@@ -825,6 +825,112 @@ def sun_visibility_backward(channels: torch.Tensor, light: torch.Tensor, sun_map
     return channels_b, map_b, light_b
 
 
+# ---- tangent-space normal maps (the model in include/deodr_b200.h) ---------------------------------------------------
+
+NORMAL_MAP_CHANNELS = 13  # the normal-mapped G-buffer: normal (3), position (3), coverage (1), tangent (3), bitangent (3)
+
+
+def uv_face_csr(faces_uv, nb_uv: int) -> Tuple[np.ndarray, np.ndarray]:
+    """The faces of every uv vertex as a CSR (offset [nb_uv+1], index [3T], int32): ascending inside a uv vertex, with
+    multiplicity, as the topology's vertex-face CSR."""
+    flat = np.ascontiguousarray(np.asarray(faces_uv), dtype=np.int64).reshape(-1)
+    if flat.size and (flat.min() < 0 or flat.max() >= nb_uv):
+        raise ValueError(f"faces_uv indices must lie in [0, {nb_uv}); got [{flat.min()}, {flat.max()}]")
+    offset = np.zeros(nb_uv + 1, dtype=np.int32)
+    np.cumsum(np.bincount(flat, minlength=nb_uv), out=offset[1:])
+    return offset, np.ascontiguousarray((np.argsort(flat, kind="stable") // 3).astype(np.int32))
+
+
+class VertexTangents:
+    """The per-vertex tangent frames (T, B) of a textured mesh (deodr_b200_vertex_tangents / _b): the faces_uv and the
+    uv-vertex-face CSR are uploaded once, beside the mesh's :class:`MeshTopology`.  Neither call synchronises with the
+    host; the adjoint is a fixed-order gather (bit-reproducible)."""
+
+    def __init__(self, topology: MeshTopology, faces_uv, nb_uv: int):
+        self.topology, self.nb_uv, self.device = topology, int(nb_uv), topology.device
+        faces_uv = np.ascontiguousarray(np.asarray(faces_uv), dtype=np.int64)
+        if faces_uv.shape != (topology.nb_faces, 3):
+            raise ValueError(f"faces_uv must be [{topology.nb_faces},3]; got {faces_uv.shape}")
+        offset, index = uv_face_csr(faces_uv, self.nb_uv)
+        self.faces_uv = torch.from_numpy(faces_uv.astype(np.uint32).view(np.int32)).to(self.device)
+        self.uv_face_offset = torch.from_numpy(offset).to(self.device)
+        self.uv_face_index = torch.from_numpy(index).to(self.device)
+
+    def _uv(self, uv: torch.Tensor) -> torch.Tensor:
+        uv = _f64(uv, self.device)
+        if tuple(uv.shape) != (self.nb_uv, 2):
+            raise ValueError(f"uv must be [{self.nb_uv},2]; got {tuple(uv.shape)}")
+        return uv
+
+    def frames(self, vertices: torch.Tensor, uv: torch.Tensor) -> torch.Tensor:
+        """-> frames [V,6] fp64 = (T_v, B_v) of ``vertices`` [V,3] and ``uv`` [Nuv,2]."""
+        vertices, uv = _f64(vertices, self.device), self._uv(uv)
+        T, V = self.topology.nb_faces, self.topology.nb_vertices
+        face_frames = torch.empty((T, 6), dtype=torch.float64, device=self.device)
+        frames = torch.empty((V, 6), dtype=torch.float64, device=self.device)
+        m = self.topology.c_struct()
+        _cabi.check(_cabi.load().deodr_b200_vertex_tangents(
+            C.byref(m), vertices.data_ptr(), self.faces_uv.data_ptr(), uv.data_ptr(), self.nb_uv,
+            face_frames.data_ptr(), frames.data_ptr(), _stream(self.device)))
+        return frames
+
+    def backward(self, vertices: torch.Tensor, uv: torch.Tensor, frames_b: torch.Tensor,
+                 vertices_b: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The adjoint of :meth:`frames` from ``frames_b`` [V,6] -> (vertices_b [V,3], accumulated into the given
+        tensor or a new zeroed one, uv_b [Nuv,2] a new tensor), fp64."""
+        vertices, uv = _f64(vertices, self.device), self._uv(uv)
+        T, V = self.topology.nb_faces, self.topology.nb_vertices
+        frames_b = _f64(frames_b, self.device)
+        if tuple(frames_b.shape) != (V, 6):
+            raise ValueError(f"frames_b must be [{V},6]; got {tuple(frames_b.shape)}")
+        if vertices_b is None:
+            vertices_b = torch.zeros((V, 3), dtype=torch.float64, device=self.device)
+        uv_b = torch.empty((self.nb_uv, 2), dtype=torch.float64, device=self.device)
+        scratch = torch.empty((6 * V + 10 * T,), dtype=torch.float64, device=self.device)
+        m = self.topology.c_struct()
+        _cabi.check(_cabi.load().deodr_b200_vertex_tangents_b(
+            C.byref(m), vertices.data_ptr(), self.faces_uv.data_ptr(), uv.data_ptr(), self.nb_uv,
+            self.uv_face_offset.data_ptr(), self.uv_face_index.data_ptr(), frames_b.data_ptr(), scratch.data_ptr(),
+            vertices_b.data_ptr(), uv_b.data_ptr(), _stream(self.device)))
+        return vertices_b, uv_b
+
+
+def _check_normal_map_io(gbuffer: torch.Tensor, nmap: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    gbuffer = gbuffer.to(dtype=torch.float32).contiguous()
+    nmap = nmap.to(device=gbuffer.device, dtype=torch.float32).contiguous()
+    if gbuffer.dim() != 3 or gbuffer.shape[2] != NORMAL_MAP_CHANNELS or tuple(nmap.shape) != tuple(gbuffer.shape[:2]) + (3,):
+        raise ValueError(f"the normal-mapped G-buffer must be [H,W,13] and the map raster [H,W,3]; got "
+                         f"{tuple(gbuffer.shape)} and {tuple(nmap.shape)}")
+    return gbuffer, nmap
+
+
+def normal_map(gbuffer: torch.Tensor, nmap: torch.Tensor) -> torch.Tensor:
+    """The perturbed G-buffer [H,W,7] = (N', X, a) f32 of a normal-mapped G-buffer ``gbuffer`` [H,W,13] = (N, X, a, T,
+    B) and the normal map's raster ``nmap`` [H,W,3] (deodr_b200_normal_map; the model in include/deodr_b200.h)."""
+    gbuffer, nmap = _check_normal_map_io(gbuffer, nmap)
+    H, W = gbuffer.shape[:2]
+    out = torch.empty((H, W, PHONG_EXTRA_CHANNELS), dtype=torch.float32, device=gbuffer.device)
+    _cabi.check(_cabi.load().deodr_b200_normal_map(gbuffer.data_ptr(), nmap.data_ptr(), H, W, out.data_ptr(),
+                                                   _stream(gbuffer.device)))
+    return out
+
+
+def normal_map_backward(gbuffer: torch.Tensor, nmap: torch.Tensor,
+                        out_b: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The adjoint of :func:`normal_map` from ``out_b`` [H,W,7] -> (gbuffer_b [H,W,13], nmap_b [H,W,3]) f32
+    (deodr_b200_normal_map_b)."""
+    gbuffer, nmap = _check_normal_map_io(gbuffer, nmap)
+    H, W = gbuffer.shape[:2]
+    out_b = out_b.to(device=gbuffer.device, dtype=torch.float32).contiguous()
+    if tuple(out_b.shape) != (H, W, PHONG_EXTRA_CHANNELS):
+        raise ValueError(f"out_b must be [{H},{W},7]; got {tuple(out_b.shape)}")
+    gbuffer_b = torch.empty_like(gbuffer)
+    nmap_b = torch.empty_like(nmap)
+    _cabi.check(_cabi.load().deodr_b200_normal_map_b(gbuffer.data_ptr(), nmap.data_ptr(), H, W, out_b.data_ptr(),
+                                                     gbuffer_b.data_ptr(), nmap_b.data_ptr(), _stream(gbuffer.device)))
+    return gbuffer_b, nmap_b
+
+
 def _light(light_directional):
     if light_directional is None:
         return None, None
@@ -1319,6 +1425,14 @@ class DeviceMeshView:
     camera's gradient with the centre's share), from one adjoint call over both rasters.  It refuses untextured views
     and ``perspective_correct``; :meth:`render_depth` and :meth:`render_deferred` are those of a textured view.
 
+    ``normal_map`` [Ht,Wt,3] (the texture's Ht and Wt; raw tangent-space vectors, x along +u, y along +v, z along the
+    outward normal) perturbs a textured Phong view's per-pixel normal (the model in include/deodr_b200.h): the G-buffer
+    gets 13 channels, the per-vertex tangent frames (T, B) after the coverage, a third raster samples the map through
+    the view's uv, and :func:`normal_map` turns the two into the 7-channel G-buffer that every shading and shadow reads.
+    The three rasters (and any shadow maps) are rendered by one renderer call and back-propagated by one;
+    :meth:`backward` adds ``normal_map_b`` [Ht,Wt,3] f32 and folds the tangent frames' share into ``vertices_b`` and
+    ``uv_b``.  ``render(..., normal_map=)`` copies a new map in.  Every other shading refuses a normal map.
+
     ``camera`` is a :class:`CameraParams`, or a camera vector [26] fp64 tensor on the view's device (extrinsic,
     intrinsic, distortion; ``has_distortion`` says whether its distortion is applied).  A tensor is read at every
     render, so a fit can update it in place between steps without a host read.  ``backward(..., camera_grad=True)``
@@ -1369,7 +1483,7 @@ class DeviceMeshView:
                  shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
                  shadow_softness: Optional[float] = None, light_shadow_map_size: int = 0,
                  light_shadow_bias: Optional[float] = None, light_shadow_softness: Optional[float] = None,
-                 light_shadow_bounds=None):
+                 light_shadow_bounds=None, normal_map=None):
         from .renderer import DeviceScene, default_renderer
         from .scenes import SceneArrays
 
@@ -1426,6 +1540,16 @@ class DeviceMeshView:
                                  f"got shape {texture.shape}")
             if uv.ndim != 2 or uv.shape[1] != 2 or faces_uv.shape != np.shape(faces):
                 raise ValueError("uv must be [Nuv,2] and faces_uv [T,3] like faces")
+        if normal_map is not None:
+            if shading != "phong_textured":
+                raise ValueError("a normal map perturbs the per-pixel normal of a textured view: it needs "
+                                 "shading='phong_textured'")
+            normal_map = np.asarray(normal_map.detach().cpu() if isinstance(normal_map, torch.Tensor) else normal_map,
+                                    dtype=np.float64)
+            if normal_map.shape != texture.shape[:2] + (3,):
+                raise ValueError(f"normal_map must be [Ht,Wt,3] with the texture's Ht and Wt = {texture.shape[:2]}; "
+                                 f"got shape {normal_map.shape}")
+        self.normal_mapped = normal_map is not None
         self.device = torch.device(device)
         self.topology = MeshTopology(faces, nb_vertices, clockwise=clockwise, device=self.device)
         self.camera, self.sigma = camera, float(sigma)
@@ -1473,10 +1597,15 @@ class DeviceMeshView:
             # the vertex colours for a textured view, whose albedo is its own raster); the coverage column is set here
             # once and never rewritten
             K = (0 if textured else nb_colors) + PHONG_EXTRA_CHANNELS
+            colors = np.concatenate((np.zeros((V, K - 1)), np.ones((V, 1))), axis=1)
+            if self.normal_mapped:
+                # (normals, positions, 1, tangents, bitangents): the coverage stays at column 6
+                K = NORMAL_MAP_CHANNELS
+                colors = np.concatenate((colors, np.zeros((V, 6))), axis=1)
             self._phong_scene = DeviceScene(SceneArrays(
                 faces=faces_u32, faces_uv=np.zeros((T, 3), np.uint32), ij=np.zeros((V, 2)), depths=np.ones(V),
                 textured=np.zeros(T, bool), uv=np.zeros((1, 2)), shade=np.zeros(V),
-                colors=np.concatenate((np.zeros((V, K - 1)), np.ones((V, 1))), axis=1), shaded=np.zeros(T, bool),
+                colors=colors, shaded=np.zeros(T, bool),
                 edgeflags=np.zeros((T, 3), bool), height=height, width=width, nb_colors=K,
                 texture=np.zeros((2, 2, K)), background_image=None, background_color=np.zeros(K), clockwise=clockwise,
                 backface_culling=bool(backface_culling), strict_edge=True, perspective_correct=False,
@@ -1484,6 +1613,15 @@ class DeviceMeshView:
             self._phong_scratch = new_scratch(self.device)
             self._phong_key = None
             self._phong_background = torch.from_numpy(background.astype(np.float32)).to(self.device)
+        if self.normal_mapped:
+            # the normal map's raster: the albedo raster's arrays with the map as a 3-channel texture
+            self._map_scene = DeviceScene(SceneArrays(
+                faces=faces_u32, faces_uv=faces_uv, ij=np.zeros((V, 2)), depths=np.ones(V), textured=flags, uv=uv,
+                shade=np.ones(V), colors=np.zeros((V, 3)), shaded=flags, edgeflags=np.zeros((T, 3), bool),
+                height=height, width=width, nb_colors=3, texture=normal_map, background_image=None,
+                background_color=np.zeros(3), clockwise=clockwise, backface_culling=bool(backface_culling),
+                strict_edge=True, perspective_correct=False, integer_pixel_centers=True), self.device)
+            self._tangents = VertexTangents(self.topology, faces_uv, uv.shape[0])
         self._maps = []  # the shadow maps rendered beside the view's raster(s): the cube maps, then the sun map
         if self.shadow_map_size:
             self._cube = ShadowCubes(faces_u32, V, point_lights.shape[0], self.shadow_map_size, clockwise, self.device)
@@ -1670,10 +1808,18 @@ class DeviceMeshView:
         return camera_gradients(camera, camera_b, self._camera_distorted, center_b)
 
     def render(self, vertices: torch.Tensor, vertex_colors: Optional[torch.Tensor] = None,
-               texture: Optional[torch.Tensor] = None) -> torch.Tensor:
+               texture: Optional[torch.Tensor] = None, normal_map: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The image [H,W,C] f32 of the mesh at ``vertices`` [V,3]: Gouraud-lit ``vertex_colors`` [V,C] for an untextured
         view; for a textured one the texture shaded by the vertex luminosity, with ``texture`` [Ht,Wt,C] (if given)
-        copied into the view's texture first, so that a fit can vary it."""
+        copied into the view's texture first, so that a fit can vary it.  ``normal_map`` [Ht,Wt,3], in a view made with
+        one, is copied into the view's normal map in the same way."""
+        if normal_map is not None:
+            if not self.normal_mapped:
+                raise ValueError("this view has no normal map (DeviceMeshView(..., normal_map=) makes one)")
+            if tuple(normal_map.shape) != tuple(self._map_scene.t["texture"].shape):
+                raise ValueError(f"normal_map has shape {tuple(normal_map.shape)}, expected "
+                                 f"{tuple(self._map_scene.t['texture'].shape)}")
+            self._map_scene.t["texture"].copy_(normal_map)
         if self.textured:
             if vertex_colors is not None:
                 raise ValueError("a textured view takes no vertex_colors (its colour is the shaded texture)")
@@ -1779,10 +1925,20 @@ class DeviceMeshView:
         g["colors"][:, 3:6].copy_(vertices)
         self.topology.edge_on_silhouette(ij, out=a["edgeflags"])
         g["edgeflags"].copy_(a["edgeflags"])
+        scenes = [self.scene, self._phong_scene]
+        if self.normal_mapped:
+            # the G-buffer's tangent and bitangent columns, and the map's raster, which shares the geometry
+            g["colors"][:, 7:13].copy_(self._tangents.frames(vertices, a["uv"]))
+            m = self._map_scene.t
+            m["ij"].copy_(ij)
+            m["depths"].copy_(depths)
+            m["edgeflags"].copy_(a["edgeflags"])
+            scenes.append(self._map_scene)
         params, center = self._phong_params()
-        fwds = self._render_with_maps([self.scene, self._phong_scene], vertices, params)
-        image, vis, sun_vis = self._shade(fwds[1]["image"], params, center, self._phong_background,
-                                          albedo=fwds[0]["image"])
+        fwds = self._render_with_maps(scenes, vertices, params)
+        gbuffer = normal_map(fwds[1]["image"], fwds[2]["image"]) if self.normal_mapped else fwds[1]["image"]
+        image, vis, sun_vis = self._shade(gbuffer, params, center, self._phong_background, albedo=fwds[0]["image"])
+        self._gbuffer = gbuffer
         self._saved = (vertices, None, normals, fwds, params, center, vis, sun_vis)
         return image
 
@@ -1791,22 +1947,39 @@ class DeviceMeshView:
         # the shading's adjoint -> albedo_b, channels_b; one adjoint call over both rasters -> texture_b, uv_b and the
         # G-buffer's colors_b (normal slice through the normal adjoint, position slice into vertices_b); the two ij_b
         # are summed before the projection's adjoint.  The albedo raster's shade_b is not used: its shade is constant
+        # with a normal map, the perturbation's adjoint first takes the 7-channel channels_b to the 13-channel
+        # G-buffer's and the map raster's image gradients; the three rasters' adjoint is one call, the tangent slices
+        # of colors_b go through the tangent frame's adjoint into vertices_b and uv_b, and the ij_b and uv_b summed
         vertices, _, _, fwds, params, center, vis, sun_vis = self._saved
-        shaded, maps_b = self._shade_backward(fwds[1]["image"], params, center, self._phong_background, image_b,
+        shaded, maps_b = self._shade_backward(self._gbuffer, params, center, self._phong_background, image_b,
                                               camera_grad, fwds[0]["image"], vis, sun_vis)
         lights_b = None
         if self.point_lights is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
         channels_b, params_b, albedo_b = shaded[0], shaded[1], shaded[-1]
-        ga, gg = self._render_b_with_maps([self.scene, self._phong_scene], fwds, [albedo_b, channels_b], maps_b)
+        scenes, image_bs = [self.scene, self._phong_scene], [albedo_b, channels_b]
+        if self.normal_mapped:
+            image_bs[1], map_image_b = normal_map_backward(fwds[1]["image"], fwds[2]["image"], channels_b)
+            scenes.append(self._map_scene)
+            image_bs.append(map_image_b)
+        grads = self._render_b_with_maps(scenes, fwds, image_bs, maps_b)
+        ga, gg = grads[:2]
         colors_b = gg["colors_b"]
         vertices_b = self.topology.vertex_normals_backward(vertices, colors_b[:, 0:3])
         vertices_b += colors_b[:, 3:6]
+        uv_b = ga["uv_b"]
+        if self.normal_mapped:
+            _, tangent_uv_b = self._tangents.backward(vertices, self.scene.t["uv"], colors_b[:, 7:13], vertices_b)
+            uv_b = (uv_b + grads[2]["uv_b"]) + tangent_uv_b.to(uv_b.dtype)
+        ij_b = ga["ij_b"] + gg["ij_b"]
+        if self.normal_mapped:
+            ij_b = ij_b + grads[2]["ij_b"]
         self._maps_backward(vertices, params, vertices_b, params_b, lights_b)
-        _, camera_b = self._project_backward(vertices, ga["ij_b"] + gg["ij_b"], None, vertices_b,
-                                             reference_transpose, camera_grad)
-        out = {"vertices_b": vertices_b, "texture_b": ga["texture_b"], "uv_b": ga["uv_b"], "light_b": params_b[:4],
+        _, camera_b = self._project_backward(vertices, ij_b, None, vertices_b, reference_transpose, camera_grad)
+        out = {"vertices_b": vertices_b, "texture_b": ga["texture_b"], "uv_b": uv_b, "light_b": params_b[:4],
                "specular_b": params_b[4:]}
+        if self.normal_mapped:
+            out["normal_map_b"] = grads[2]["texture_b"]
         if camera_grad:
             out.update(self._camera_result(camera_b, shaded[2]))
         if self.sh is not None:
@@ -1843,7 +2016,7 @@ class DeviceMeshView:
         e_b) for a Phong view, sh_b for a view with an environment and point_lights_b for a view with point lights;
         for a textured view
         dict(vertices_b, texture_b [Ht,Wt,C] f32, uv_b [Nuv,2] f32, light_b), plus specular_b for a textured Phong
-        view: the luminosity's adjoint ``shade_b`` goes
+        view (and normal_map_b [Ht,Wt,3] f32 for a normal-mapped one): the luminosity's adjoint ``shade_b`` goes
         through the luminosity and normal adjoints, ``ij_b`` through the projection's.  With ``camera_grad`` the dict
         also holds extrinsic_b, intrinsic_b and distortion_b (see the class); it refuses ``reference_transpose``."""
         if camera_grad and reference_transpose:

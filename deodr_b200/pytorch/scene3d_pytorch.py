@@ -32,7 +32,9 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
                            point_lights [L, 3 + S] | None get theirs
     RenderMeshPhongTexturedFunc  (ij, uv, texture, channels [V,7], depths, edgeflags, albedo scene, G-buffer scene,
                            sigma) -> (albedo [H,W,C], G-buffer [H,W,7]): the two rasters of a textured Phong render
-                           in one forward call and one adjoint call; gradients to ij, uv, texture and channels
+                           in one forward call and one adjoint call; gradients to ij, uv, texture and channels.  With
+                           a normal map [Ht,Wt,3] and its scene, channels are [V,13] and a third raster, the map's
+                           [H,W,3], is rendered in the same calls; the map receives its gradient
     RenderShadowedPhongFunc  (ij, uv | None, texture | None, channels, depths, edgeflags, vertices, point_lights,
                            albedo scene | None, G-buffer scene, ShadowCubes, sigma) -> ([albedo,] G-buffer, cube maps
                            [6L,M,M]): a Phong render's raster(s) and the lights' cube shadow maps in one forward call
@@ -42,6 +44,10 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
     SunVisibilityFunc      (G-buffer, light_directional [3], map [M,M], bounds, bias, softness, albedo | None) ->
                            visibility [H,W] of the directional light; the G-buffer, the map and the light receive
                            their gradients
+    VertexTangentsFunc     (vertices [V,3], uv [Nuv,2], VertexTangents) -> frames [V,6] = (T, B), the per-vertex
+                           tangent frames of a normal-mapped mesh; the vertices and the uv receive their gradients
+    NormalMapFunc          (G-buffer [H,W,13], map raster [H,W,3]) -> G-buffer [H,W,7], the normal map's per-pixel
+                           perturbation; both inputs receive their gradients
 
 All maths is fp64 but the rasteriser's (fp32 image and image gradients).  ``RenderMesh2DFunc``,
 ``RenderMesh2DTexturedFunc`` and ``RenderMeshPhongTexturedFunc`` follow the snapshot / replay rule of the 2D Functions (differentiable_renderer_pytorch.py):
@@ -65,7 +71,8 @@ from ..mesh_ops import (CameraParams, LoopSubdivision, MeshTopology, camera_cent
                         shadow_visibility_backward,
                         point_lit_vertex_colors, point_lit_vertex_colors_backward, sh_lit_vertex_colors,
                         sh_lit_vertex_colors_backward,
-                        project_points_backward_f64, project_points_camera_backward, project_points_dev)
+                        project_points_backward_f64, project_points_camera_backward, project_points_dev,
+                        VertexTangents, normal_map, normal_map_backward)
 from ..renderer import DeviceScene, default_renderer
 from .differentiable_renderer_pytorch import check_scene_inputs, gradients_of, requested_grads
 
@@ -334,42 +341,59 @@ class RenderMeshPhongTexturedFunc(torch.autograd.Function):
     @staticmethod
     def forward(ctx: Any, ij: torch.Tensor, uv: torch.Tensor, texture: torch.Tensor,  # type: ignore
                 channels: torch.Tensor, depths: torch.Tensor, edgeflags: torch.Tensor, albedo_scene: DeviceScene,
-                gbuffer_scene: DeviceScene, sigma: float = 1.0):
+                gbuffer_scene: DeviceScene, sigma: float = 1.0, normal_map: Optional[torch.Tensor] = None,
+                map_scene: Optional[DeviceScene] = None):
+        if (normal_map is None) != (map_scene is None):
+            raise ValueError("a normal map comes with its scene")
         check_scene_inputs(albedo_scene, uv=uv, texture=texture)
         check_scene_inputs(gbuffer_scene, colors=channels)
-        inputs = (ij.detach(), uv.detach(), texture.detach(), channels.detach(), depths.detach(), edgeflags)
-        RenderMeshPhongTexturedFunc._update(albedo_scene, gbuffer_scene, *inputs)
-        fwds = default_renderer(albedo_scene.device.index).render_views([albedo_scene, gbuffer_scene], sigma)
-        ctx.scenes, ctx.sigma, ctx.fwds = (albedo_scene, gbuffer_scene), float(sigma), fwds
-        ctx.in_dtypes = (ij.dtype, uv.dtype, texture.dtype, channels.dtype)
-        ctx.save_for_backward(*(t.clone() for t in inputs))
+        scenes = [albedo_scene, gbuffer_scene]
+        if map_scene is not None:
+            check_scene_inputs(map_scene, uv=uv, texture=normal_map)
+            scenes.append(map_scene)
+        inputs = (ij.detach(), uv.detach(), texture.detach(), channels.detach(), depths.detach(), edgeflags,
+                  normal_map.detach() if normal_map is not None else None)
+        RenderMeshPhongTexturedFunc._update(scenes, *inputs)
+        fwds = default_renderer(albedo_scene.device.index).render_views(scenes, sigma)
+        ctx.scenes, ctx.sigma, ctx.fwds = scenes, float(sigma), fwds
+        ctx.in_dtypes = (ij.dtype, uv.dtype, texture.dtype, channels.dtype,
+                         normal_map.dtype if normal_map is not None else None)
+        ctx.save_for_backward(*(t.clone() if t is not None else None for t in inputs))
         # the caller gets its own tensors: the framebuffers of ctx.fwds may be re-rendered into by backward
-        return fwds[0]["image"].clone(), fwds[1]["image"].clone()
+        return tuple(f["image"].clone() for f in fwds)
 
     @staticmethod
-    def _update(albedo_scene, gbuffer_scene, ij, uv, texture, channels, depths, edgeflags) -> None:
-        albedo_scene.update(ij=ij, uv=uv, texture=texture, depths=depths, edgeflags=edgeflags)
-        gbuffer_scene.update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
+    def _update(scenes, ij, uv, texture, channels, depths, edgeflags, normal_map) -> None:
+        scenes[0].update(ij=ij, uv=uv, texture=texture, depths=depths, edgeflags=edgeflags)
+        scenes[1].update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
+        if len(scenes) > 2:
+            scenes[2].update(ij=ij, uv=uv, texture=normal_map, depths=depths, edgeflags=edgeflags)
 
     @staticmethod
-    def backward(ctx: Any, albedo_b: torch.Tensor, gbuffer_b: torch.Tensor):  # type: ignore
-        needs = ctx.needs_input_grad[:4]
+    def backward(ctx: Any, *image_bs):  # type: ignore
+        needs = ctx.needs_input_grad[:4] + ctx.needs_input_grad[9:10]
         if not any(needs):
-            return (None,) * 9
-        albedo_scene, gbuffer_scene = ctx.scenes
-        renderer = default_renderer(albedo_scene.device.index)
+            return (None,) * 11
+        scenes = ctx.scenes
+        renderer = default_renderer(scenes[0].device.index)
         # the shared scenes may hold another node's inputs by now
-        RenderMeshPhongTexturedFunc._update(albedo_scene, gbuffer_scene, *ctx.saved_tensors)
+        RenderMeshPhongTexturedFunc._update(scenes, *ctx.saved_tensors)
         if any(f["generation"] != renderer.generation(f["slot"]) for f in ctx.fwds):
-            ctx.fwds = renderer.render_views([albedo_scene, gbuffer_scene], ctx.sigma, out=ctx.fwds)
-        ga = requested_grads(albedo_scene, RenderMeshPhongTexturedFunc.NAMES, (needs[0], needs[1], False, needs[2]))
-        gg = gbuffer_scene.zero_grads()
-        renderer.render_b_views([albedo_scene, gbuffer_scene], ctx.sigma, ctx.fwds,
-                                [albedo_b.contiguous(), gbuffer_b.contiguous()], grads=[ga, gg])
-        ij_d, uv_d, tex_d, ch_d = ctx.in_dtypes
-        return ((ga["ij_b"] + gg["ij_b"]).to(ij_d) if needs[0] else None, ga["uv_b"].to(uv_d) if needs[1] else None,
+            ctx.fwds = renderer.render_views(scenes, ctx.sigma, out=ctx.fwds)
+        names = RenderMeshPhongTexturedFunc.NAMES
+        grads = [requested_grads(scenes[0], names, (needs[0], needs[1], False, needs[2])), scenes[1].zero_grads()]
+        if len(scenes) > 2:
+            grads.append(requested_grads(scenes[2], names, (needs[0], needs[1], False, needs[4])))
+        renderer.render_b_views(scenes, ctx.sigma, ctx.fwds, [b.contiguous() for b in image_bs], grads=grads)
+        ga, gg = grads[:2]
+        ij_d, uv_d, tex_d, ch_d, nm_d = ctx.in_dtypes
+        ij_b, uv_b = ga["ij_b"] + gg["ij_b"], ga["uv_b"]
+        if len(scenes) > 2:
+            ij_b, uv_b = ij_b + grads[2]["ij_b"], uv_b + grads[2]["uv_b"]
+        return (ij_b.to(ij_d) if needs[0] else None, uv_b.to(uv_d) if needs[1] else None,
                 ga["texture_b"].to(tex_d) if needs[2] else None, gg["colors_b"].to(ch_d) if needs[3] else None,
-                None, None, None, None, None)
+                None, None, None, None, None,
+                grads[2]["texture_b"].to(nm_d) if len(scenes) > 2 and needs[4] else None, None)
 
 
 class PoseFunc(torch.autograd.Function):
@@ -541,25 +565,35 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
                 channels: torch.Tensor, depths: torch.Tensor, edgeflags: torch.Tensor, vertices: torch.Tensor,
                 point_lights: Optional[torch.Tensor], albedo_scene: Optional[DeviceScene], gbuffer_scene: DeviceScene,
                 cubes: Optional[ShadowCubes], sigma: float = 1.0, light_directional: Optional[torch.Tensor] = None,
-                sun: Optional[SunShadowMap] = None):
+                sun: Optional[SunShadowMap] = None, normal_map: Optional[torch.Tensor] = None,
+                map_scene: Optional[DeviceScene] = None):
         textured = albedo_scene is not None
         if textured:
             check_scene_inputs(albedo_scene, uv=uv, texture=texture)
         check_scene_inputs(gbuffer_scene, colors=channels)
         if (cubes is None) != (point_lights is None) or (sun is None) != (light_directional is None):
             raise ValueError("the cube maps come with point_lights, and the sun map with light_directional")
+        mapped = map_scene is not None
+        if (normal_map is None) != (not mapped) or (mapped and not textured):
+            raise ValueError("a normal map comes with its scene, in a textured render")
+        if mapped:
+            check_scene_inputs(map_scene, uv=uv, texture=normal_map)
         inputs = (ij.detach(), uv.detach() if textured else None, texture.detach() if textured else None,
                   channels.detach(), depths.detach(), edgeflags, _f64(vertices.detach()),
                   _f64(point_lights.detach()) if cubes is not None else None,
-                  _f64(light_directional.detach()).reshape(3).contiguous() if sun is not None else None)
-        ctx.scenes = ([albedo_scene] if textured else []) + [gbuffer_scene]
+                  _f64(light_directional.detach()).reshape(3).contiguous() if sun is not None else None,
+                  normal_map.detach() if mapped else None)
+        # the rasters: [albedo,] G-buffer[, normal map]
+        ctx.scenes = ([albedo_scene] if textured else []) + [gbuffer_scene] + ([map_scene] if mapped else [])
+        ctx.gi = 1 if textured else 0
         ctx.maps = [m for m in (cubes, sun) if m is not None]
-        ctx.cubes, ctx.sun, ctx.sigma, ctx.textured = cubes, sun, float(sigma), textured
+        ctx.cubes, ctx.sun, ctx.sigma, ctx.textured, ctx.mapped = cubes, sun, float(sigma), textured, mapped
         renderer = default_renderer(gbuffer_scene.device.index)
         ctx.fwds = RenderShadowedPhongFunc._render(renderer, ctx, inputs, None)
         ctx.in_dtypes = (ij.dtype, uv.dtype if textured else None, texture.dtype if textured else None, channels.dtype,
                          vertices.dtype, point_lights.dtype if cubes is not None else None,
-                         light_directional.dtype if sun is not None else None)
+                         light_directional.dtype if sun is not None else None,
+                         normal_map.dtype if mapped else None)
         ctx.save_for_backward(*(t.clone() if t is not None else None for t in inputs))
         rasters = tuple(f["image"].clone() for f in ctx.fwds[:len(ctx.scenes)])
         return rasters + ((cubes.maps.clone(),) if cubes is not None else ()) + \
@@ -573,12 +607,18 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
             ctx.sun.prepare(inputs[6], inputs[8])
 
     @staticmethod
-    def _render(renderer, ctx, inputs, out):
+    def _update(ctx, inputs):
         ij, uv, texture, channels, depths, edgeflags = inputs[:6]
         if ctx.textured:
             ctx.scenes[0].update(ij=ij, uv=uv, texture=texture, depths=depths, edgeflags=edgeflags)
-        ctx.scenes[-1].update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
+        ctx.scenes[ctx.gi].update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
+        if ctx.mapped:
+            ctx.scenes[2].update(ij=ij, uv=uv, texture=inputs[9], depths=depths, edgeflags=edgeflags)
         RenderShadowedPhongFunc._prepare(ctx, inputs)
+
+    @staticmethod
+    def _render(renderer, ctx, inputs, out):
+        RenderShadowedPhongFunc._update(ctx, inputs)
         if out is None:
             out = [renderer._new_outputs(sc, False, False, False) for sc in ctx.scenes] + \
                 [o for m in ctx.maps for o in m.outputs()]
@@ -587,23 +627,22 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx: Any, *grads):  # type: ignore
         needs = ctx.needs_input_grad
-        if not any(needs[:8]) and not needs[12]:
-            return (None,) * 14
+        if not any(needs[:8]) and not needs[12] and not needs[14]:
+            return (None,) * 16
         inputs = ctx.saved_tensors
-        renderer = default_renderer(ctx.scenes[-1].device.index)
+        renderer = default_renderer(ctx.scenes[ctx.gi].device.index)
         n = len(ctx.scenes)
         # the shared scenes and maps may hold another node's inputs by now
         if any(f["generation"] != renderer.generation(f["slot"]) for f in ctx.fwds):
             ctx.fwds = RenderShadowedPhongFunc._render(renderer, ctx, inputs, ctx.fwds)
         else:
-            if ctx.textured:
-                ctx.scenes[0].update(ij=inputs[0], uv=inputs[1], texture=inputs[2], depths=inputs[4],
-                                     edgeflags=inputs[5])
-            ctx.scenes[-1].update(ij=inputs[0], colors=inputs[3], depths=inputs[4], edgeflags=inputs[5])
-            RenderShadowedPhongFunc._prepare(ctx, inputs)
+            RenderShadowedPhongFunc._update(ctx, inputs)
         if ctx.textured:
             gs = [requested_grads(ctx.scenes[0], RenderShadowedPhongFunc.NAMES, (True, needs[1], False, needs[2])),
                   ctx.scenes[1].zero_grads()]
+            if ctx.mapped:
+                gs.append(requested_grads(ctx.scenes[2], RenderShadowedPhongFunc.NAMES,
+                                          (True, needs[1], False, needs[14])))
         else:
             gs = [ctx.scenes[0].zero_grads()]
         image_bs = [g.to(torch.float32).contiguous() for g in grads[:n]]
@@ -623,15 +662,17 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
         if ctx.sun is not None:
             _, light_b = sun_project_backward(inputs[6], inputs[8], ctx.sun.bounds, ctx.sun.M, ctx.sun.ij_b[0],
                                               ctx.sun.colors_b.view(-1), scratch, vertices_b=vertices_b)
-        ij_d, uv_d, tex_d, ch_d, v_d, l_d, d_d = ctx.in_dtypes
+        ij_d, uv_d, tex_d, ch_d, v_d, l_d, d_d, nm_d = ctx.in_dtypes
         ij_b = sum(g["ij_b"] for g in gs)
+        uv_b = gs[0]["uv_b"] + gs[2]["uv_b"] if ctx.mapped else gs[0]["uv_b"]
         return (ij_b.to(ij_d) if needs[0] else None,
-                gs[0]["uv_b"].to(uv_d) if ctx.textured and needs[1] else None,
+                uv_b.to(uv_d) if ctx.textured and needs[1] else None,
                 gs[0]["texture_b"].to(tex_d) if ctx.textured and needs[2] else None,
-                gs[-1]["colors_b"].to(ch_d) if needs[3] else None, None, None,
+                gs[ctx.gi]["colors_b"].to(ch_d) if needs[3] else None, None, None,
                 vertices_b.to(v_d) if needs[6] else None,
                 lights_b.to(l_d) if lights_b is not None and needs[7] else None,
-                None, None, None, None, light_b.to(d_d) if light_b is not None and needs[12] else None, None)
+                None, None, None, None, light_b.to(d_d) if light_b is not None and needs[12] else None, None,
+                gs[2]["texture_b"].to(nm_d) if ctx.mapped and needs[14] else None, None)
 
 
 class ShadowVisibilityFunc(torch.autograd.Function):
@@ -695,6 +736,46 @@ class SunVisibilityFunc(torch.autograd.Function):
                 map_b.to(md) if needs[2] else None, None, None, None, None)
 
 
+class VertexTangentsFunc(torch.autograd.Function):
+    """The per-vertex tangent frames of a normal-mapped mesh (deodr_b200_vertex_tangents / _b, the model in
+    include/deodr_b200.h): (vertices [V,3], uv [Nuv,2], VertexTangents) -> frames [V,6] = (T, B) fp64.  Backward
+    returns the gradients of the vertices and the uv, each a fixed-order gather."""
+
+    @staticmethod
+    def forward(ctx: Any, vertices: torch.Tensor, uv: torch.Tensor, tangents: VertexTangents):  # type: ignore
+        v, w = _f64(vertices), _f64(uv)
+        ctx.save_for_backward(v, w)
+        ctx.tangents, ctx.dtypes = tangents, (vertices.dtype, uv.dtype)
+        return tangents.frames(v, w)
+
+    @staticmethod
+    def backward(ctx: Any, frames_b: torch.Tensor):  # type: ignore
+        v, w = ctx.saved_tensors
+        vertices_b, uv_b = ctx.tangents.backward(v, w, frames_b)
+        needs = ctx.needs_input_grad
+        return (vertices_b.to(ctx.dtypes[0]) if needs[0] else None, uv_b.to(ctx.dtypes[1]) if needs[1] else None,
+                None)
+
+
+class NormalMapFunc(torch.autograd.Function):
+    """The normal map's per-pixel perturbation (deodr_b200_normal_map / _b, the model in include/deodr_b200.h):
+    (G-buffer [H,W,13] = (N, X, a, T, B), map raster [H,W,3]) -> G-buffer [H,W,7] = (N', X, a) fp32."""
+
+    @staticmethod
+    def forward(ctx: Any, gbuffer: torch.Tensor, nmap: torch.Tensor):  # type: ignore
+        g, m = gbuffer.detach().to(torch.float32).contiguous(), nmap.detach().to(torch.float32).contiguous()
+        ctx.save_for_backward(g, m)
+        ctx.dtypes = (gbuffer.dtype, nmap.dtype)
+        return normal_map(g, m)
+
+    @staticmethod
+    def backward(ctx: Any, out_b: torch.Tensor):  # type: ignore
+        g, m = ctx.saved_tensors
+        g_b, m_b = normal_map_backward(g, m, out_b)
+        needs = ctx.needs_input_grad
+        return g_b.to(ctx.dtypes[0]) if needs[0] else None, m_b.to(ctx.dtypes[1]) if needs[1] else None
+
+
 project_points_autograd = ProjectPointsFunc.apply
 vertex_normals_autograd = VertexNormalsFunc.apply
 lit_vertex_colors_autograd = LitVertexColorsFunc.apply
@@ -710,6 +791,8 @@ phong_shade_autograd = PhongShadeFunc.apply
 render_shadowed_phong = RenderShadowedPhongFunc.apply
 shadow_visibility_autograd = ShadowVisibilityFunc.apply
 sun_visibility_autograd = SunVisibilityFunc.apply
+vertex_tangents_autograd = VertexTangentsFunc.apply
+normal_map_autograd = NormalMapFunc.apply
 
 
 def vertex_luminosity_autograd(normals: torch.Tensor, light_directional: Optional[torch.Tensor],
@@ -793,10 +876,14 @@ class ColoredTriMeshPytorch:
     ``faces_uv`` [T,3], ``uv`` [Nuv,2] and ``texture`` [Ht,Wt,C], given together, make the mesh textured, in the
     conventions of the reference's ``ColoredTriMesh`` (uv in texel units).  ``uv`` and ``texture`` are tensors (fp32 or
     fp64, either may require grad) or arrays, uploaded once; the attributes ``uv`` and ``texture`` may be reassigned
-    between renders."""
+    between renders.
+
+    ``normal_map`` [Ht,Wt,3] (a textured mesh's, with the texture's Ht and Wt; a tensor that may require grad, or an
+    array) is a tangent-space normal map, read by ``Scene3DPytorch(shading="phong_textured")`` (the model in
+    include/deodr_b200.h); the attribute may be reassigned between renders."""
 
     def __init__(self, faces, vertices, clockwise: bool = False, colors=None, device=None, faces_uv=None, uv=None,
-                 texture=None):
+                 texture=None, normal_map=None):
         self.device = _device(device if device is not None else
                               (vertices.device if isinstance(vertices, torch.Tensor) else None))
         self.faces = np.ascontiguousarray(np.asarray(faces), dtype=np.int64)
@@ -823,6 +910,23 @@ class ColoredTriMeshPytorch:
             # the rasteriser reads uv through faces_uv unchecked
             if self.faces_uv.size and (self.faces_uv.min() < 0 or self.faces_uv.max() >= self.uv.shape[0]):
                 raise ValueError(f"faces_uv indices must lie in [0, {self.uv.shape[0]})")
+        self.normal_map = None
+        self._tangents: Optional[VertexTangents] = None
+        if normal_map is not None:
+            if not self.textured:
+                raise ValueError("a normal map is addressed by the uv: it needs a textured mesh")
+            self.normal_map = self._tensor(normal_map)
+            if tuple(self.normal_map.shape) != tuple(self.texture.shape[:2]) + (3,):
+                raise ValueError(f"normal_map must be [Ht,Wt,3] with the texture's Ht and Wt = "
+                                 f"{tuple(self.texture.shape[:2])}; got {tuple(self.normal_map.shape)}")
+
+    @property
+    def tangents(self) -> VertexTangents:
+        """The mesh's :class:`~deodr_b200.mesh_ops.VertexTangents` (faces_uv and the uv-vertex-face CSR on the device),
+        built on first use."""
+        if self._tangents is None:
+            self._tangents = VertexTangents(self.topology, self.faces_uv, self.uv.shape[0])
+        return self._tangents
 
     @property
     def textured(self) -> bool:
@@ -882,7 +986,9 @@ class Scene3DPytorch:
     ``shading="phong_textured"`` lights a textured mesh per pixel: the albedo raster (the texture with a shade of 1
     over a zero background) and a G-buffer ``[normals | vertices | 1]`` are rendered by one
     :class:`RenderMeshPhongTexturedFunc` node and shaded by :class:`PhongShadeFunc` with the albedo apart; grey and
-    coloured environments apply.
+    coloured environments apply.  A mesh with a ``normal_map`` adds its tangent frames (:class:`VertexTangentsFunc`)
+    to the G-buffer and the map's raster to the same node, and :class:`NormalMapFunc` perturbs the G-buffer's normal
+    before the shading and the shadows read it; the map, the uv and the vertices receive their gradients.
 
     ``set_point_lights`` adds point lights near the mesh in every shading; a table that requires grad receives its
     gradient, and the vertices receive the lights' share through their normals and their positions.  A flash is a
@@ -1022,14 +1128,15 @@ class Scene3DPytorch:
                 integer_pixel_centers=True), m.device)
         return self._scenes[key]
 
-    def _phong_scene(self, camera: CameraPytorch, nb_colors: int) -> DeviceScene:
-        """The cached G-buffer scene of the mesh for ``camera``: C + 7 channels, zero background."""
+    def _phong_scene(self, camera: CameraPytorch, nb_colors: int, normal_mapped: bool = False) -> DeviceScene:
+        """The cached G-buffer scene of the mesh for ``camera``: C + 7 channels (13 for a normal-mapped textured mesh),
+        zero background."""
         from ..scenes import SceneArrays
 
-        key = (camera.height, camera.width, nb_colors)
+        key = (camera.height, camera.width, nb_colors + (6 if normal_mapped else 0))
         if key not in self._phong_scenes:
             m = self.mesh
-            T, V, K = m.nb_faces, m.nb_vertices, nb_colors + 7
+            T, V, K = m.nb_faces, m.nb_vertices, key[2] + 7
             faces = np.ascontiguousarray(m.faces, dtype=np.uint32)
             self._phong_scenes[key] = DeviceScene(SceneArrays(
                 faces=faces, faces_uv=faces, ij=np.zeros((V, 2)), depths=np.ones(V), textured=np.zeros(T, bool),
@@ -1040,12 +1147,14 @@ class Scene3DPytorch:
                 perspective_correct=False, integer_pixel_centers=True), m.device)
         return self._phong_scenes[key]
 
-    def _albedo_scene(self, camera: CameraPytorch, uv: torch.Tensor, texture: torch.Tensor) -> DeviceScene:
-        """The cached albedo raster of a textured mesh for ``camera``: all triangles textured and shaded, a shade of 1
-        at every vertex (set here once), colours zero, zero background."""
+    def _albedo_scene(self, camera: CameraPytorch, uv: torch.Tensor, texture: torch.Tensor,
+                      normal_map: bool = False) -> DeviceScene:
+        """The cached albedo raster of a textured mesh for ``camera`` (with ``normal_map``, the normal map's raster, its
+        texture the map): all triangles textured and shaded, a shade of 1 at every vertex (set here once), colours zero,
+        zero background."""
         from ..scenes import SceneArrays
 
-        key = (camera.height, camera.width, tuple(texture.shape), uv.shape[0])
+        key = (camera.height, camera.width, tuple(texture.shape), uv.shape[0], normal_map)
         if key not in self._albedo_scenes:
             m = self.mesh
             T, V, nc = m.nb_faces, m.nb_vertices, texture.shape[2]
@@ -1072,16 +1181,32 @@ class Scene3DPytorch:
         ij, depths = camera.project_points(m.vertices)
         ones = torch.ones((m.nb_vertices, 1), dtype=torch.float64, device=m.device)
         channels = torch.cat((m.vertex_normals, m.vertices.to(torch.float64), ones), dim=1)
+        nmap = map_scene = None
+        if m.normal_map is not None:
+            # (normals, positions, 1, tangents, bitangents), and the map's raster beside the albedo's
+            nmap = m._tensor(m.normal_map)
+            if tuple(nmap.shape) != tuple(texture.shape[:2]) + (3,):
+                raise ValueError(f"normal_map must be [Ht,Wt,3] with the texture's Ht and Wt = "
+                                 f"{tuple(texture.shape[:2])}; got {tuple(nmap.shape)}")
+            channels = torch.cat((channels, vertex_tangents_autograd(m.vertices, uv, m.tangents)), dim=1)
+            map_scene = self._albedo_scene(camera, uv, nmap, normal_map=True)
         vis = sun = None
         if self.shadow_map_size or self.light_shadow_map_size:
             out = self._render_shadowed(ij, uv, texture, channels, depths, self._albedo_scene(camera, uv, texture),
-                                        self._phong_scene(camera, 0))
+                                        self._phong_scene(camera, 0, nmap is not None), nmap, map_scene)
+            rasters = 3 if nmap is not None else 2
             albedo, gbuffer = out[:2]
-            vis, sun = self._visibilities(gbuffer, out[2:], albedo)
+            if nmap is not None:
+                gbuffer = normal_map_autograd(gbuffer, out[2])
+            vis, sun = self._visibilities(gbuffer, out[rasters:], albedo)
         else:
-            albedo, gbuffer = render_mesh_phong_textured(ij, uv, texture, channels, depths, self._edgeflags(ij),
-                                                         self._albedo_scene(camera, uv, texture),
-                                                         self._phong_scene(camera, 0), self.sigma)
+            out = render_mesh_phong_textured(ij, uv, texture, channels, depths, self._edgeflags(ij),
+                                             self._albedo_scene(camera, uv, texture),
+                                             self._phong_scene(camera, 0, nmap is not None), self.sigma, nmap,
+                                             map_scene)
+            albedo, gbuffer = out[:2]
+            if nmap is not None:
+                gbuffer = normal_map_autograd(gbuffer, out[2])
         return phong_shade_autograd(gbuffer, self.light_directional, self.light_ambient, self.specular,
                                     self.shininess, camera.center() if camera.is_tensor else camera,
                                     self.background_color, self.light_sh, albedo, self.point_lights, vis, sun)
@@ -1112,14 +1237,16 @@ class Scene3DPytorch:
                                     camera.center() if camera.is_tensor else camera, self.background_color,
                                     self.light_sh, None, self.point_lights, vis, sun)
 
-    def _render_shadowed(self, ij, uv, texture, channels, depths, albedo_scene, gbuffer_scene) -> tuple:
+    def _render_shadowed(self, ij, uv, texture, channels, depths, albedo_scene, gbuffer_scene, normal_map=None,
+                         map_scene=None) -> tuple:
         """The rasters and the shadow maps in one :class:`RenderShadowedPhongFunc` node."""
         m = self.mesh
         cubes = self._shadow_cubes() if self.shadow_map_size else None
         sun = self._sun_map() if self.light_shadow_map_size else None
         return render_shadowed_phong(ij, uv, texture, channels, depths, self._edgeflags(ij), m.vertices,
                                      self.point_lights if cubes is not None else None, albedo_scene, gbuffer_scene,
-                                     cubes, self.sigma, self.light_directional if sun is not None else None, sun)
+                                     cubes, self.sigma, self.light_directional if sun is not None else None, sun,
+                                     normal_map, map_scene)
 
     def _visibilities(self, gbuffer, maps, albedo) -> tuple:
         """(the point lights' visibility or None, the directional light's or None) from the node's maps."""

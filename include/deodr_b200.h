@@ -809,6 +809,64 @@ int deodr_b200_phong_shade_sun_shadowed_b(const DeodrPhongIO *io, const float *a
                                           float *vis_b, const float *sun_vis, float *sun_vis_b, double *scratch,
                                           void *stream);
 
+/* ---- tangent-space normal maps (textured Phong) -------------------------------------------------------------------
+ * A normal map [Ht, Wt, 3] fp32 has the albedo texture's Ht and Wt and is addressed by the same uv / faces_uv (texel
+ * units, shifted by -0.5).  Its texels are raw tangent-space vectors (not [0, 1]-encoded: the caller decodes 8-bit
+ * maps): x along +u (texture columns), y along +v (texture rows, downwards), z along the outward normal.  A map in the
+ * OpenGL convention has its y negated by the caller.
+ *
+ * Per-vertex tangent frame.  Face f with position ids (i0, i1, i2) and uv ids (k0, k1, k2):
+ *   e1 = x_i1 - x_i0,  e2 = x_i2 - x_i0,  (du1, dv1) = uv_k1 - uv_k0,  (du2, dv2) = uv_k2 - uv_k0
+ *   det = du1 dv2 - du2 dv1,  sigma = sign(det) (0 when det = 0)
+ *   t_f = sigma (dv2 e1 - dv1 e2),  b_f = sigma (du1 e2 - du2 e1)      (|det| dx/du and |det| dx/dv: uv-area weights)
+ *   T_v = normalize(sum_{f ∋ v} t_f),  B_v = normalize(sum_{f ∋ v} b_f)  (0 for a zero sum)
+ * The sums run over the topology's vertex-face CSR, in its order, as deodr_b200_vertex_normals's.
+ *
+ * G-buffer.  A normal-mapped view rasterises 13 channels per vertex, (N, X, 1, T, B), and a third raster, the normal
+ * map sampled like the albedo (shade 1, zero background, 3 channels), M; all three share the view's geometry.  Per
+ * pixel, with coverage a:
+ *   a = 0:  N' = 0 (nothing else is read; every gradient is 0)
+ *   n  = N / |N|                          (0 when |N| = 0)
+ *   t~ = T - <T, n> n,  t = t~ / |t~|     (0 when |t~| = 0)
+ *   b~ = n x t,  s = +1 if <b~, B> >= 0 else -1,  b = s b~
+ *   p  = (M_x t + M_y b) + M_z n          (summed in that order)
+ *   N' = a p / |p|                        (0 when |p| = 0)
+ * M carries the coverage as a factor, which normalising p cancels.  The result is the 7-channel G-buffer (N', X, a)
+ * of DeodrPhongIO's albedo form, which every shading and visibility entry point reads unchanged.
+ *
+ * Adjoint: N'_b goes to N_b, T_b, M_b and a_b (B_b = 0: s is piecewise constant, as sigma is); the X and a slices
+ * pass through.  The rasteriser's adjoint of the three rasters then gives the G-buffer's colors_b, whose T and B slices
+ * go to deodr_b200_vertex_tangents_b, and the map's texture_b.  Every sum is a gather in a fixed order (no atomics),
+ * so the tangents' adjoint is bit-reproducible.
+ *
+ * Limitations: a vertex shared by mirrored uv charts gets cancelling tangents (the caller splits such vertices); the
+ * frame is not MikkTSpace, so maps baked by other tools may shade slightly differently; sampling is the rasteriser's
+ * bilinear sampling, without mip levels; at self-occlusion silhouettes the frame is the mixed frame of the Phong
+ * G-buffer.
+ *
+ * Caller contract: faces_uv indexes [0, nb_uv) and the topology's faces [0, V); neither can be checked on the device
+ * without a host synchronisation, so neither is.  None of these calls synchronises with the host. */
+
+/* face_frames [T,6] = (t_f, b_f) and frames [V,6] = (T_v, B_v), fp64, overwritten, from vertices [V,3] fp64, faces_uv
+ * [T,3] and uv [nb_uv,2] fp64.  DEODR_B200_EINVAL before any launch for a NULL buffer (the topology's faces and its
+ * vertex-face CSR included) or T, V or nb_uv < 1. */
+int deodr_b200_vertex_tangents(const DeodrMeshTopology *mesh, const double *vertices, const uint32_t *faces_uv,
+                               const double *uv, int nb_uv, double *face_frames, double *frames, void *stream);
+/* Its adjoint from frames_b [V,6] fp64: vertices_b [V,3] fp64 accumulated, one thread per position vertex; uv_b
+ * [nb_uv,2] fp64 overwritten, one thread per uv vertex walking the uv-vertex-face CSR (uv_face_offset [nb_uv+1],
+ * uv_face_index [3T]: the faces of every uv vertex, ascending, with multiplicity, as the topology's vertex-face CSR).
+ * scratch: 6 V + 10 T doubles.  Same refusals, plus a NULL CSR, scratch or output. */
+int deodr_b200_vertex_tangents_b(const DeodrMeshTopology *mesh, const double *vertices, const uint32_t *faces_uv,
+                                 const double *uv, int nb_uv, const int32_t *uv_face_offset,
+                                 const int32_t *uv_face_index, const double *frames_b, double *scratch,
+                                 double *vertices_b, double *uv_b, void *stream);
+/* out [H,W,7] = (N', X, a) from gbuffer [H,W,13] = (N, X, a, T, B) and the map raster map [H,W,3], fp32, one thread
+ * per pixel, fp64 maths.  DEODR_B200_EINVAL before any launch for a NULL buffer or H or W < 1. */
+int deodr_b200_normal_map(const float *gbuffer, const float *map, int H, int W, float *out, void *stream);
+/* Its adjoint from out_b [H,W,7]: gbuffer_b [H,W,13] and map_b [H,W,3] fp32, overwritten.  Same refusals. */
+int deodr_b200_normal_map_b(const float *gbuffer, const float *map, int H, int W, const float *out_b,
+                            float *gbuffer_b, float *map_b, void *stream);
+
 /* One parameter vector of a heavy-ball update (device pointers, `size` entries each):
  *   step = clamp(-grad * factor, -max_step, max_step)   (max_step = INFINITY: unclamped)
  *   speed = (1 - damping) (speed * inertia + (1 - inertia) step);  value += speed
