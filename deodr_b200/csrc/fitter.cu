@@ -838,14 +838,18 @@ constexpr int PHONG_SUMS = 6;  // l_b (3), ambient_b, ks_b, e_b; then camera_cen
 
 // The shading terms of one pixel, kept for the adjoint.  `lit`: |l| > 0 (else the normals are not read); `spec_on`:
 // lit and a != 0; `s` is max(0, <n, h>) and p = s^e (0 at s = 0).
+// With a specular map (SPEC), `sp` is the pixel's (K, E) of the map raster and the term uses aks = ks K and
+// e(p) = e E / a, kept in `aks` and `e` (set only where spec_on).
 struct PhongTerms {
     double n[3], nn, dot_nl, lum;
     double a, ll, u[3], x[3], v[3], dn, h[3], hn, s, p, spec;
+    double aks, e;
     bool lit, spec_on;
 };
 
+template <bool SPEC = false>
 __device__ __forceinline__ void phong_terms(const float *px, const DeodrPhongIO &io, const double *prm,
-                                            const double *cam, PhongTerms &t) {
+                                            const double *cam, PhongTerms &t, const float *sp = nullptr) {
     const double N[3] = {px[io.off_normal], px[io.off_normal + 1], px[io.off_normal + 2]};
     const double l[3] = {prm[0], prm[1], prm[2]};
     t.nn = sqrt(dot(N, N));
@@ -873,8 +877,15 @@ __device__ __forceinline__ void phong_terms(const float *px, const DeodrPhongIO 
     for (int j = 0; j < 3; j++) t.h[j] = t.hn == 0.0 ? 0.0 : hh[j] / t.hn;
     const double s = dot(t.n, t.h);
     t.s = s > 0 ? s : 0.0;
-    t.p = t.s > 0 ? pow(t.s, prm[5]) : 0.0;
-    t.spec = ((t.a * prm[4]) * t.ll) * t.p;
+    if constexpr (SPEC) {
+        t.aks = prm[4] * (double)sp[0];
+        t.e = prm[5] * ((double)sp[1] / t.a);
+        t.p = t.s > 0 ? pow(t.s, t.e) : 0.0;
+        t.spec = (t.aks * t.ll) * t.p;
+    } else {
+        t.p = t.s > 0 ? pow(t.s, prm[5]) : 0.0;
+        t.spec = ((t.a * prm[4]) * t.ll) * t.p;
+    }
 }
 
 // Where the albedo A of pixel p is read and its adjoint written: the G-buffer's slice at off_albedo (a G-buffer of
@@ -903,18 +914,22 @@ __device__ __forceinline__ float &albedo_b_at(float *pb, const DeodrPhongIO &io,
 // the luminosity and Q_c to the specular term (P = 1: grey); at P = 3 the default budget spills 12 bytes across the
 // pow calls, so the point-light instances take one CTA's registers too (DESIGN.md section 13).  With VIS (P > 0), light
 // j's diffuse and specular terms are multiplied by its visibility vis [H,W,L] (DESIGN.md section 14); with SUN, the
-// directional light's by sun_vis [H,W] (DESIGN.md section 15)
-template <int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false>
+// directional light's by sun_vis [H,W] (DESIGN.md section 15).  With SPEC (SPLIT only), the specular map's
+// raster spec_map [H,W,2] = (K, E) gives every specular term, the point lights' included, aks = ks K and e(p) =
+// e E / a in place of a ks and e (DESIGN.md section 17)
+template <int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false, bool SPEC = false>
 __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(DeodrPhongIO io, const double *sh,
                                                                   const float *albedo, const double *lights, int L,
                                                                   const float *vis = nullptr,
-                                                                  const float *sun_vis = nullptr) {
+                                                                  const float *sun_vis = nullptr,
+                                                                  const float *spec_map = nullptr) {
+    static_assert(SPLIT || !SPEC, "a specular map is read beside a separate albedo");
     const long long p = (long long)blockIdx.x * NT + threadIdx.x;
     if (p >= (long long)io.H * io.W) return;
     const int C = io.C;
     const float *px = io.channels + p * gbuffer_stride<SPLIT>(C);
     PhongTerms t;
-    phong_terms(px, io, io.params, io.camera_center, t);
+    phong_terms<SPEC>(px, io, io.params, io.camera_center, t, SPEC ? spec_map + 2 * p : nullptr);
     if constexpr (SUN) {
         // each product rounded on its own, so that V = 1 leaves the terms, and the image, bit for bit
         const double sv = sun_vis[p];
@@ -936,7 +951,8 @@ __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(Deod
             }
             const double dn = sqrt(dot(v, v));
             for (int j = 0; j < 3; j++) v[j] /= dn;
-            const double aks = t.a * io.params[4], e = io.params[5];
+            const double aks = SPEC ? io.params[4] * (double)spec_map[2 * p] : t.a * io.params[4];
+            const double e = SPEC ? io.params[5] * ((double)spec_map[2 * p + 1] / t.a) : io.params[5];
             for (int j = 0; j < L; j++) {
                 const double *lj = lights + j * (3 + P);
                 PointTerm pt;
@@ -997,11 +1013,16 @@ __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(Deod
 // (0 where a = 0).  With SUN, the directional diff and spec are scaled by sun_vis [H,W] and sun_vis_b[p] =
 // sum_c g_c (A_c diff + spec) is written; at S = 3 without point lights the default budget spills then too, so
 // those take one CTA's registers (DESIGN.md section 15).
-template <bool CENTER, int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false>
-__global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P == 0) ? 1 : 0)
+// With SPEC (SPLIT only), aks = ks K and e(p) = e E / a from spec_map [H,W,2] = (K, E): q and e_b(p), the
+// gradients of aks and e(p) summed over the main term and the point lights, give spec_map_b [H,W,2] = (q ks,
+// e_b(p) e / a) (0 where a = 0), ks_b += q K, e_b += e_b(p) E / a and a_b -= e_b(p) e(p) / a (DESIGN.md section 17).
+template <bool CENTER, int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false, bool SPEC = false>
+__global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P == 0) || SPEC ? 1 : 0)
     k_phong_shade_b(DeodrPhongIO io, Scratch *s, const double *sh, const float *albedo, float *albedo_b,
                     const double *lights, int L, const float *vis = nullptr, float *vis_b = nullptr,
-                    const float *sun_vis = nullptr, float *sun_vis_b = nullptr) {
+                    const float *sun_vis = nullptr, float *sun_vis_b = nullptr, const float *spec_map = nullptr,
+                    float *spec_map_b = nullptr) {
+    static_assert(SPLIT || !SPEC, "a specular map is read beside a separate albedo");
     constexpr int NC = S > P ? S : P;
     constexpr int K = PHONG_SUMS + (CENTER ? 3 : 0);
     __shared__ double tot[K];
@@ -1049,6 +1070,7 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
         // camera centre's into acc.  alpha_j = sum_c g_c A_c I_j[c] and beta_j = sum_c g_c I_j[c] are the gradients of
         // the light's diffuse and specular factors.
         double pd[P > 0 ? P : 1], pX_b[3] = {0, 0, 0}, pa_b = 0;
+        double sq = 0, se_b = 0;  // with SPEC: the gradients of aks and e(p), summed over the terms
         if constexpr (P > 0) {
 #pragma unroll
             for (int c = 0; c < P; c++) pd[c] = 0;
@@ -1077,12 +1099,13 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
                         gs[0] += g[c];
                     }
                 }
-                const double aks = a * ks;
+                const double aks = SPEC ? ks * (double)spec_map[2 * p] : a * ks;
+                const double ep = SPEC ? e * ((double)spec_map[2 * p + 1] / a) : e;
                 double v_b[3] = {0, 0, 0}, x_b[3] = {0, 0, 0}, q = 0, e_b = 0;
                 for (int j = 0; j < L; j++) {
                     const double *lj = lights + j * (3 + P);
                     PointTerm pt;
-                    point_term(lj, x, n, true, v, aks, e, pt);
+                    point_term(lj, x, n, true, v, aks, ep, pt);
                     double alpha = 0, beta = 0, d_b[3] = {0, 0, 0}, vj = 1.0;
                     if constexpr (VIS) vj = vis[p * L + j];
                     const double diff = VIS ? __dmul_rn(pt.diff, vj) : pt.diff;
@@ -1097,12 +1120,17 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
                         alpha = __dmul_rn(alpha, vj);
                         beta = __dmul_rn(beta, vj);
                     }
-                    point_term_b(pt, n, alpha, beta, aks, e, n_b, d_b, v_b, q, e_b);
+                    point_term_b(pt, n, alpha, beta, aks, ep, n_b, d_b, v_b, q, e_b);
                     for (int k = 0; k < 3; k++) x_b[k] -= d_b[k];
                 }
-                acc[4] += q * a;
-                acc[5] += e_b;
-                pa_b = q * ks;
+                if constexpr (SPEC) {
+                    sq = q;
+                    se_b = e_b;
+                } else {
+                    acc[4] += q * a;
+                    acc[5] += e_b;
+                    pa_b = q * ks;
+                }
                 double dv_b[3] = {0, 0, 0};
                 normalize_b(v, v_b, dn, dv_b);  // v = normalize(cam - x)
                 for (int j = 0; j < 3; j++) {
@@ -1116,7 +1144,7 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
             }
         }
         PhongTerms t;
-        phong_terms(px, io, prm, io.camera_center, t);
+        phong_terms<SPEC>(px, io, prm, io.camera_center, t, SPEC ? spec_map + 2 * p : nullptr);
         double sv = 1.0, diff0 = 0, spec0 = 0;  // with SUN: V and the unshadowed directional terms
         if constexpr (SUN) {
             sv = sun_vis[p];
@@ -1165,14 +1193,24 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
                 acc[j] -= diff_b * t.n[j];
             }
         if (t.spec_on) {
-            a_b += spec_b * ((ks * t.ll) * t.p);
-            acc[4] += spec_b * ((t.a * t.ll) * t.p);
-            const double ll_b = spec_b * ((t.a * ks) * t.p);
+            double ll_b;
+            if constexpr (SPEC) {
+                sq += spec_b * (t.ll * t.p);
+                ll_b = spec_b * (t.aks * t.p);
+            } else {
+                a_b += spec_b * ((ks * t.ll) * t.p);
+                acc[4] += spec_b * ((t.a * t.ll) * t.p);
+                ll_b = spec_b * ((t.a * ks) * t.p);
+            }
             for (int j = 0; j < 3; j++) acc[j] += ll_b * t.u[j];
             if (t.s > 0) {
-                const double p_b = spec_b * ((t.a * ks) * t.ll);
-                const double s_b = p_b * e * pow(t.s, e - 1);
-                acc[5] += p_b * t.p * log(t.s);
+                const double p_b = spec_b * (SPEC ? t.aks * t.ll : (t.a * ks) * t.ll);
+                const double ep = SPEC ? t.e : e;
+                const double s_b = p_b * ep * pow(t.s, ep - 1);
+                if constexpr (SPEC)
+                    se_b += p_b * t.p * log(t.s);
+                else
+                    acc[5] += p_b * t.p * log(t.s);
                 double h_b[3];
                 for (int j = 0; j < 3; j++) {
                     n_b[j] += s_b * t.h[j];
@@ -1191,6 +1229,20 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
                     }
                     a_b += dot(d_b, t.x) / t.a;
                 }
+            }
+        }
+        if constexpr (SPEC) {
+            // aks = ks K and e(p) = e E / a: the map's gradient, ks_b and e_b, and e(p)'s share of a_b
+            float *sb = spec_map_b + 2 * p;
+            if (t.a != 0.0) {
+                const double K = spec_map[2 * p], E = spec_map[2 * p + 1];
+                sb[0] = (float)(sq * ks);
+                sb[1] = (float)(se_b * e / t.a);
+                acc[4] += sq * K;
+                acc[5] += se_b * E / t.a;
+                a_b -= se_b * (e * (E / t.a)) / t.a;
+            } else {
+                sb[0] = sb[1] = 0.0f;
             }
         }
         if ((t.lit || S > 0 || P > 0) && t.nn != 0.0) normalize_b(t.n, n_b, t.nn, N_b);
@@ -1246,11 +1298,13 @@ __global__ void __launch_bounds__(NT) k_phong_sh_b(DeodrPhongIO io, Scratch *s, 
 // lights_b [L, 3 + P] of the Phong forms: CTA (j, y) sums light j over a fixed set of pixels, the position's gradient
 // (the d_j share of k_phong_shade_b) and the intensity's, g_c A_c diff_j + g_c spec_j (P = 1: summed over the
 // channels); grid_sum_rows adds the CTAs in a fixed order.  The CTAs of one set of pixels are adjacent in the grid, so
-// the G-buffer is read from DRAM about once.  With VIS, light j's terms are scaled by vis [H,W,L].
-template <int P, bool SPLIT, bool VIS = false>
+// the G-buffer is read from DRAM about once.  With VIS, light j's terms are scaled by vis [H,W,L].  With SPEC, the
+// terms use aks = ks K and e(p) = e E / a from spec_map [H,W,2]; the map's gradient is k_phong_shade_b's.
+template <int P, bool SPLIT, bool VIS = false, bool SPEC = false>
 __global__ void __launch_bounds__(NT) k_point_lights_pixel_b(DeodrPhongIO io, const float *albedo,
                                                              const double *lights, double *lights_b, Scratch *s,
-                                                             const float *vis = nullptr) {
+                                                             const float *vis = nullptr,
+                                                             const float *spec_map = nullptr) {
     constexpr int K = 3 + P;
     const double *lj = lights + blockIdx.x * K;
     double acc[K];
@@ -1287,8 +1341,10 @@ __global__ void __launch_bounds__(NT) k_point_lights_pixel_b(DeodrPhongIO io, co
                 gs[0] += g[c];
             }
         }
+        const double aks = SPEC ? ks * (double)spec_map[2 * p] : a * ks;
+        const double ep = SPEC ? e * ((double)spec_map[2 * p + 1] / a) : e;
         PointTerm pt;
-        point_term(lj, x, n, true, v, a * ks, e, pt);
+        point_term(lj, x, n, true, v, aks, ep, pt);
         double alpha = 0, beta = 0, d_b[3] = {0, 0, 0}, n_b[3] = {0, 0, 0}, v_b[3] = {0, 0, 0}, q = 0, e_b = 0;
 #pragma unroll
         for (int c = 0; c < P; c++) {
@@ -1301,7 +1357,7 @@ __global__ void __launch_bounds__(NT) k_point_lights_pixel_b(DeodrPhongIO io, co
             alpha = __dmul_rn(alpha, vj);
             beta = __dmul_rn(beta, vj);
         }
-        point_term_b(pt, n, alpha, beta, a * ks, e, n_b, d_b, v_b, q, e_b);
+        point_term_b(pt, n, alpha, beta, aks, ep, n_b, d_b, v_b, q, e_b);
         for (int k = 0; k < 3; k++) acc[k] += d_b[k];
         const double diff = VIS ? __dmul_rn(pt.diff, vj) : pt.diff, spec = VIS ? __dmul_rn(pt.spec, vj) : pt.spec;
 #pragma unroll
@@ -1391,18 +1447,18 @@ void launch_sh_lit_b(const double *normals, const double *vcol, int n, int C, co
                                                      sh_b, s);
 }
 
-template <int S, bool SPLIT = false, bool SUN = false>
+template <int S, bool SPLIT = false, bool SUN = false, bool SPEC = false>
 void launch_phong_b(const DeodrPhongIO &io, const double *sh, double *sh_b, Scratch *s, cudaStream_t st,
                     const float *albedo = nullptr, float *albedo_b = nullptr, const float *sun_vis = nullptr,
-                    float *sun_vis_b = nullptr) {
+                    float *sun_vis_b = nullptr, const float *spec_map = nullptr, float *spec_map_b = nullptr) {
     const long long pixels = (long long)io.H * io.W;
     const int g = reduce_grid(pixels);
     if (io.camera_center_b)
-        k_phong_shade_b<true, S, SPLIT, 0, false, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, nullptr, 0,
-                                                                         nullptr, nullptr, sun_vis, sun_vis_b);
+        k_phong_shade_b<true, S, SPLIT, 0, false, SUN, SPEC><<<g, NT, 0, st>>>(
+            io, s, sh, albedo, albedo_b, nullptr, 0, nullptr, nullptr, sun_vis, sun_vis_b, spec_map, spec_map_b);
     else
-        k_phong_shade_b<false, S, SPLIT, 0, false, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, nullptr, 0,
-                                                                          nullptr, nullptr, sun_vis, sun_vis_b);
+        k_phong_shade_b<false, S, SPLIT, 0, false, SUN, SPEC><<<g, NT, 0, st>>>(
+            io, s, sh, albedo, albedo_b, nullptr, 0, nullptr, nullptr, sun_vis, sun_vis_b, spec_map, spec_map_b);
     if constexpr (S > 0)
         k_phong_sh_b<S, SPLIT><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo);
 }
@@ -1446,23 +1502,25 @@ dim3 light_grid(long long items, int L, int P) {
     return dim3(L, std::max(1, std::min(reduce_grid(items), MAX_K * MAX_CTAS / (L * (3 + P)))));
 }
 
-template <int S, int P, bool SPLIT, bool VIS = false, bool SUN = false>
+template <int S, int P, bool SPLIT, bool VIS = false, bool SUN = false, bool SPEC = false>
 void launch_point_phong_b(const DeodrPhongIO &io, const float *albedo, float *albedo_b, const double *sh,
                           double *sh_b, const double *lights, int L, double *lights_b, Scratch *s, cudaStream_t st,
                           const float *vis = nullptr, float *vis_b = nullptr, const float *sun_vis = nullptr,
-                          float *sun_vis_b = nullptr) {
+                          float *sun_vis_b = nullptr, const float *spec_map = nullptr, float *spec_map_b = nullptr) {
     const long long pixels = (long long)io.H * io.W;
     const int g = reduce_grid(pixels);
     if (io.camera_center_b)
-        k_phong_shade_b<true, S, SPLIT, P, VIS, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis,
-                                                                       vis_b, sun_vis, sun_vis_b);
+        k_phong_shade_b<true, S, SPLIT, P, VIS, SUN, SPEC><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L,
+                                                                             vis, vis_b, sun_vis, sun_vis_b, spec_map,
+                                                                             spec_map_b);
     else
-        k_phong_shade_b<false, S, SPLIT, P, VIS, SUN><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L, vis,
-                                                                        vis_b, sun_vis, sun_vis_b);
+        k_phong_shade_b<false, S, SPLIT, P, VIS, SUN, SPEC><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L,
+                                                                              vis, vis_b, sun_vis, sun_vis_b, spec_map,
+                                                                              spec_map_b);
     if constexpr (S > 0)
         k_phong_sh_b<S, SPLIT><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo);
-    k_point_lights_pixel_b<P, SPLIT, VIS><<<light_grid(pixels, L, P), NT, 0, st>>>(io, albedo, lights, lights_b, s,
-                                                                                   vis);
+    k_point_lights_pixel_b<P, SPLIT, VIS, SPEC><<<light_grid(pixels, L, P), NT, 0, st>>>(io, albedo, lights, lights_b,
+                                                                                         s, vis, spec_map);
 }
 
 }  // namespace
@@ -1990,6 +2048,82 @@ int deodr_b200_phong_shade_sun_shadowed_b(const DeodrPhongIO *io, const float *a
             else
                 launch_point_phong_b<S, P, false, VIS, true>(*io, nullptr, nullptr, sh, sh_b, lights, nb_lights,
                                                              lights_b, s, st, vis, vis_b, sun_vis, sun_vis_b);
+        });
+    });
+    return check_launch();
+}
+
+int deodr_b200_phong_shade_specular_map(const DeodrPhongIO *io, const float *albedo, const float *spec,
+                                        const double *sh, int sh_channels, const double *lights, int nb_lights,
+                                        int light_channels, const float *vis, const float *sun_vis, void *stream) {
+    if (!phong_io_ok(io, true) || !io->image || !albedo || !spec || (!sh && sh_channels != 0) ||
+        (!lights && (nb_lights != 0 || vis)))
+        return bad("phong_shade_specular_map: bad argument (H, W >= 1, C in [1, 32760], off_albedo -1 and the other "
+                   "offsets tiling [0, 7), channels, params, camera_center, background, image, albedo and spec "
+                   "non-NULL, sh NULL only with sh_channels 0, lights NULL only with nb_lights 0 and no vis)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) ||
+        (lights && (!light_channels_ok(light_channels, io->C) || nb_lights < 1 || nb_lights > MAX_LIGHTS)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "phong_shade_specular_map: nb_lights must be 1 to 8, and "
+                                                  "sh_channels and light_channels 1, or C from 1 to 4");
+    const int g = grid_of((long long)io->H * io->W);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S_ = sh ? sh_channels : 0;
+    if (!lights) {
+        with_sh_channels(S_, [&](auto S) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                k_phong_shade<S, true, 0, false, SUN, true><<<g, NT, 0, st>>>(*io, sh, albedo, nullptr, 0, nullptr,
+                                                                              sun_vis, spec);
+            });
+        });
+        return check_launch();
+    }
+    with_point_channels(S_, light_channels, [&](auto S, auto P) {
+        with_flag(vis != nullptr, [&](auto VIS) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                k_phong_shade<S, true, P, VIS, SUN, true><<<g, NT, 0, st>>>(*io, sh, albedo, lights, nb_lights, vis,
+                                                                            sun_vis, spec);
+            });
+        });
+    });
+    return check_launch();
+}
+
+int deodr_b200_phong_shade_specular_map_b(const DeodrPhongIO *io, const float *albedo, const float *spec,
+                                          const double *sh, int sh_channels, const double *lights, int nb_lights,
+                                          int light_channels, const float *vis, const float *sun_vis,
+                                          float *albedo_b, float *spec_b, double *sh_b, double *lights_b,
+                                          float *vis_b, float *sun_vis_b, double *scratch, void *stream) {
+    if (!phong_io_ok(io, true) || !io->image_b || !io->channels_b || !io->params_b || !albedo || !albedo_b ||
+        !spec || !spec_b || (!sh && sh_channels != 0) || (sh && !sh_b) || (!lights && (nb_lights != 0 || vis)) ||
+        (lights && !lights_b) || (vis && !vis_b) || (sun_vis && !sun_vis_b) || !scratch)
+        return bad("phong_shade_specular_map_b: bad argument (H, W >= 1, C in [1, 32760], off_albedo -1 and the "
+                   "other offsets tiling [0, 7), channels, params, camera_center, background, image_b, channels_b, "
+                   "params_b, albedo, albedo_b, spec, spec_b and scratch non-NULL, sh NULL only with sh_channels 0, "
+                   "sh_b non-NULL with sh, lights NULL only with nb_lights 0 and no vis, lights_b non-NULL with "
+                   "lights, vis_b with vis, sun_vis_b with sun_vis)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) ||
+        (lights && (!light_channels_ok(light_channels, io->C) || nb_lights < 1 || nb_lights > MAX_LIGHTS)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "phong_shade_specular_map_b: nb_lights must be 1 to 8, and "
+                                                  "sh_channels and light_channels 1, or C from 1 to 4");
+    Scratch *s = reinterpret_cast<Scratch *>(scratch);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S_ = sh ? sh_channels : 0;
+    if (!lights) {
+        with_sh_channels(S_, [&](auto S) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                launch_phong_b<S, true, SUN, true>(*io, sh, sh_b, s, st, albedo, albedo_b, sun_vis, sun_vis_b, spec,
+                                                   spec_b);
+            });
+        });
+        return check_launch();
+    }
+    with_point_channels(S_, light_channels, [&](auto S, auto P) {
+        with_flag(vis != nullptr, [&](auto VIS) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                launch_point_phong_b<S, P, true, VIS, SUN, true>(*io, albedo, albedo_b, sh, sh_b, lights, nb_lights,
+                                                                 lights_b, s, st, vis, vis_b, sun_vis, sun_vis_b,
+                                                                 spec, spec_b);
+            });
         });
     });
     return check_launch();

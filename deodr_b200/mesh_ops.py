@@ -423,11 +423,21 @@ def _phong_io(channels: torch.Tensor, params: torch.Tensor, center: torch.Tensor
     return io, (channels, params, center, background, albedo)
 
 
+def _check_specular(spec: torch.Tensor, albedo: Optional[torch.Tensor], H: int, W: int, device) -> torch.Tensor:
+    """The specular map's raster [H,W,2] as a contiguous f32 tensor on ``device``; it needs the separate albedo."""
+    if albedo is None:
+        raise ValueError("a specular map's raster is read beside a separate albedo (a textured Phong view's)")
+    if not isinstance(spec, torch.Tensor) or tuple(spec.shape) != (H, W, 2):
+        raise ValueError(f"specular must be an [{H},{W},2] tensor; got {tuple(getattr(spec, 'shape', ()))}")
+    return spec.to(device=device, dtype=torch.float32).contiguous()
+
+
 def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: torch.Tensor,
                 background: torch.Tensor, sh: Optional[torch.Tensor] = None,
                 albedo: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None,
                 visibility: Optional[torch.Tensor] = None,
-                sun_visibility: Optional[torch.Tensor] = None) -> torch.Tensor:
+                sun_visibility: Optional[torch.Tensor] = None,
+                specular: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The per-pixel shading of a G-buffer (deodr_b200_phong_shade, or deodr_b200_sh_phong_shade with ``sh``; model in
     include/deodr_b200.h): ``channels``
     [H,W,C+7] f32 laid out (albedo C, normal 3, position 3, coverage 1), ``params`` [6] fp64 on the device = (light
@@ -439,12 +449,26 @@ def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: tor
     lights, the lights' visibility [H,W,L] f32 (:func:`shadow_visibility`), which multiplies each light's diffuse and
     specular terms (deodr_b200_point_phong_shade_shadowed).  ``sun_visibility``: the directional light's visibility
     [H,W] f32 (:func:`sun_visibility`), which multiplies its diffuse and specular terms, with or without an
-    environment, point lights and their ``visibility`` (deodr_b200_phong_shade_sun_shadowed)."""
+    environment, point lights and their ``visibility`` (deodr_b200_phong_shade_sun_shadowed).  ``specular``: with an
+    albedo, the specular map's raster [H,W,2] = (K, E) (the model in include/deodr_b200.h), which gives every specular
+    term aks = ks K and e(p) = e E / a, with any of the inputs above (deodr_b200_phong_shade_specular_map)."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     H, W = keep[0].shape[:2]
     image = torch.empty((H, W, io.C), dtype=torch.float32, device=keep[0].device)
     io.image = image.data_ptr()
-    if sun_visibility is not None:
+    if specular is not None:
+        spec = _check_specular(specular, albedo, H, W, image.device)
+        sun = _check_sun_visibility(sun_visibility, H, W, image.device) if sun_visibility is not None else None
+        lights, L, P = _check_point_lights(point_lights, image.device) if point_lights is not None else (None, 0, 0)
+        vis = _check_visibility(visibility, H, W, L, image.device) if visibility is not None else None
+        if vis is not None and lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        sh, S = _check_sh(sh, image.device) if sh is not None else (None, 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        _cabi.check(_cabi.load().deodr_b200_phong_shade_specular_map(
+            C.byref(io), keep[4].data_ptr(), spec.data_ptr(), ptr(sh), S, ptr(lights), L, P, ptr(vis), ptr(sun),
+            _stream(image.device)))
+    elif sun_visibility is not None:
         sun = _check_sun_visibility(sun_visibility, H, W, image.device)
         lights, L, P = _check_point_lights(point_lights, image.device) if point_lights is not None else (None, 0, 0)
         vis = _check_visibility(visibility, H, W, L, image.device) if visibility is not None else None
@@ -490,7 +514,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
                          albedo: Optional[torch.Tensor] = None,
                          point_lights: Optional[torch.Tensor] = None,
                          visibility: Optional[torch.Tensor] = None,
-                         sun_visibility: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
+                         sun_visibility: Optional[torch.Tensor] = None,
+                         specular: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
     """-> (channels_b [H,W,C+7] f32, params_b [6] fp64), the adjoint of :func:`phong_shade` from ``image_b`` [H,W,C]
     (deodr_b200_phong_shade_b, or deodr_b200_sh_phong_shade_b with ``sh``).  channels_b includes the coverage channel's gradient; ``params_b`` is summed over the
     pixels in a fixed order (bit-reproducible).  ``scratch``: a buffer of ``mesh_fitter.new_scratch``.  With
@@ -500,7 +525,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     (deodr_b200_phong_shade_albedo_b).  With ``point_lights`` the result ends with lights_b [L, 3 + S] fp64, summed
     in a fixed order (deodr_b200_point_phong_shade_b); with ``visibility`` too it then ends with vis_b [H,W,L] f32
     (deodr_b200_point_phong_shade_shadowed_b).  With ``sun_visibility`` the result ends with sun_vis_b [H,W] f32
-    (deodr_b200_phong_shade_sun_shadowed_b)."""
+    (deodr_b200_phong_shade_sun_shadowed_b).  With ``specular`` (the map raster of :func:`phong_shade`) it ends with
+    spec_b [H,W,2] f32 (deodr_b200_phong_shade_specular_map_b)."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     dev = keep[0].device
     S = _check_sh(sh, dev)[1] if sh is not None else 0
@@ -519,8 +545,23 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
     if albedo is not None:
         albedo_b = torch.empty((H, W, io.C), dtype=torch.float32, device=dev)
-    lights_b = vis_b = sun_b = None
-    if sun_visibility is not None:
+    lights_b = vis_b = sun_b = spec_b = None
+    if specular is not None:
+        spec = _check_specular(specular, albedo, H, W, dev)
+        sun = _check_sun_visibility(sun_visibility, H, W, dev) if sun_visibility is not None else None
+        lights, L, P = _check_point_lights(point_lights, dev) if point_lights is not None else (None, 0, 0)
+        vis = _check_visibility(visibility, H, W, L, dev) if visibility is not None else None
+        if vis is not None and lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        lights_b = torch.empty_like(lights) if lights is not None else None
+        vis_b = torch.empty((H, W, L), dtype=torch.float32, device=dev) if vis is not None else None
+        sun_b = torch.empty((H, W), dtype=torch.float32, device=dev) if sun is not None else None
+        spec_b = torch.empty((H, W, 2), dtype=torch.float32, device=dev)
+        _cabi.check(_cabi.load().deodr_b200_phong_shade_specular_map_b(
+            C.byref(io), keep[4].data_ptr(), spec.data_ptr(), ptr(sh), S, ptr(lights), L, P, ptr(vis), ptr(sun),
+            albedo_b.data_ptr(), spec_b.data_ptr(), ptr(sh_b), ptr(lights_b), ptr(vis_b), ptr(sun_b),
+            scratch.data_ptr(), _stream(dev)))
+    elif sun_visibility is not None:
         sun = _check_sun_visibility(sun_visibility, H, W, dev)
         lights, L, P = _check_point_lights(point_lights, dev) if point_lights is not None else (None, 0, 0)
         vis = _check_visibility(visibility, H, W, L, dev) if visibility is not None else None
@@ -563,7 +604,8 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     out = out if albedo_b is None else out + (albedo_b,)
     out = out if lights_b is None else out + (lights_b,)
     out = out if vis_b is None else out + (vis_b,)
-    return out if sun_b is None else out + (sun_b,)
+    out = out if sun_b is None else out + (sun_b,)
+    return out if spec_b is None else out + (spec_b,)
 
 
 # ---- shadows from point lights (the model in include/deodr_b200.h) ---------------------------------------------------
@@ -1433,6 +1475,13 @@ class DeviceMeshView:
     :meth:`backward` adds ``normal_map_b`` [Ht,Wt,3] f32 and folds the tangent frames' share into ``vertices_b`` and
     ``uv_b``.  ``render(..., normal_map=)`` copies a new map in.  Every other shading refuses a normal map.
 
+    ``specular_map`` [Ht,Wt,2] (the texture's Ht and Wt) varies a textured Phong view's highlight per texel (the model
+    in include/deodr_b200.h): texel (ks_t, e_t) multiplies ``specular`` and ``shininess``, so a map of ones is the view
+    without a map.  One more raster samples the map through the view's uv, rendered and back-propagated in the same
+    renderer calls as the others (and any shadow maps), and the shading reads it per pixel.  :meth:`backward` adds
+    ``specular_map_b`` [Ht,Wt,2] f32 and the map raster's share of ``uv_b`` and of the vertices' gradient.
+    ``render(..., specular_map=)`` copies a new map in.  Every other shading refuses a specular map.
+
     ``camera`` is a :class:`CameraParams`, or a camera vector [26] fp64 tensor on the view's device (extrinsic,
     intrinsic, distortion; ``has_distortion`` says whether its distortion is applied).  A tensor is read at every
     render, so a fit can update it in place between steps without a host read.  ``backward(..., camera_grad=True)``
@@ -1483,7 +1532,7 @@ class DeviceMeshView:
                  shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
                  shadow_softness: Optional[float] = None, light_shadow_map_size: int = 0,
                  light_shadow_bias: Optional[float] = None, light_shadow_softness: Optional[float] = None,
-                 light_shadow_bounds=None, normal_map=None):
+                 light_shadow_bounds=None, normal_map=None, specular_map=None):
         from .renderer import DeviceScene, default_renderer
         from .scenes import SceneArrays
 
@@ -1550,6 +1599,16 @@ class DeviceMeshView:
                 raise ValueError(f"normal_map must be [Ht,Wt,3] with the texture's Ht and Wt = {texture.shape[:2]}; "
                                  f"got shape {normal_map.shape}")
         self.normal_mapped = normal_map is not None
+        if specular_map is not None:
+            if shading != "phong_textured":
+                raise ValueError("a specular map varies the per-pixel highlight of a textured view: it needs "
+                                 "shading='phong_textured'")
+            specular_map = np.asarray(specular_map.detach().cpu() if isinstance(specular_map, torch.Tensor)
+                                      else specular_map, dtype=np.float64)
+            if specular_map.shape != texture.shape[:2] + (2,):
+                raise ValueError(f"specular_map must be [Ht,Wt,2] with the texture's Ht and Wt = {texture.shape[:2]}; "
+                                 f"got shape {specular_map.shape}")
+        self.specular_mapped = specular_map is not None
         self.device = torch.device(device)
         self.topology = MeshTopology(faces, nb_vertices, clockwise=clockwise, device=self.device)
         self.camera, self.sigma = camera, float(sigma)
@@ -1622,6 +1681,14 @@ class DeviceMeshView:
                 background_color=np.zeros(3), clockwise=clockwise, backface_culling=bool(backface_culling),
                 strict_edge=True, perspective_correct=False, integer_pixel_centers=True), self.device)
             self._tangents = VertexTangents(self.topology, faces_uv, uv.shape[0])
+        if self.specular_mapped:
+            # the specular map's raster: the albedo raster's arrays with the map as a 2-channel texture
+            self._spec_scene = DeviceScene(SceneArrays(
+                faces=faces_u32, faces_uv=faces_uv, ij=np.zeros((V, 2)), depths=np.ones(V), textured=flags, uv=uv,
+                shade=np.ones(V), colors=np.zeros((V, 2)), shaded=flags, edgeflags=np.zeros((T, 3), bool),
+                height=height, width=width, nb_colors=2, texture=specular_map, background_image=None,
+                background_color=np.zeros(2), clockwise=clockwise, backface_culling=bool(backface_culling),
+                strict_edge=True, perspective_correct=False, integer_pixel_centers=True), self.device)
         self._maps = []  # the shadow maps rendered beside the view's raster(s): the cube maps, then the sun map
         if self.shadow_map_size:
             self._cube = ShadowCubes(faces_u32, V, point_lights.shape[0], self.shadow_map_size, clockwise, self.device)
@@ -1699,9 +1766,11 @@ class DeviceMeshView:
             self._sun.backward(vertices, params, vertices_b, params_b, self._phong_scratch)
 
     def _shade(self, gbuffer: torch.Tensor, params: torch.Tensor, center: torch.Tensor, background: torch.Tensor,
-               albedo: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
-        """phong_shade of a G-buffer, under the point lights' and the directional light's visibility in a view with
-        shadows -> (image, vis or None, sun_vis or None)."""
+               albedo: Optional[torch.Tensor] = None,
+               spec: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """phong_shade of a G-buffer (with the specular map's raster ``spec`` in a view with a map), under the point
+        lights' and the directional light's visibility in a view with shadows -> (image, vis or None, sun_vis or
+        None)."""
         vis = sun_vis = None
         if self.shadow_map_size:
             vis = shadow_visibility(gbuffer, self.point_lights, self._cube.maps, self.shadow_bias,
@@ -1710,15 +1779,21 @@ class DeviceMeshView:
             sun_vis = sun_visibility(gbuffer, params, self._sun.map, self.light_shadow_bounds, self.light_shadow_bias,
                                      self.light_shadow_softness, albedo=albedo)
         return phong_shade(gbuffer, params, center, background, sh=self.sh, albedo=albedo,
-                           point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis), vis, sun_vis
+                           point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis,
+                           specular=spec), vis, sun_vis
 
-    def _shade_backward(self, gbuffer, params, center, background, image_b, camera_grad, albedo, vis, sun_vis):
+    def _shade_backward(self, gbuffer, params, center, background, image_b, camera_grad, albedo, vis, sun_vis,
+                        spec=None):
         """phong_shade_backward, and in a view with shadows the visibilities' adjoints added into channels_b, lights_b
-        and params_b -> (the result of phong_shade_backward without vis_b and sun_vis_b, the maps' gradients in the
-        order of self._maps)."""
+        and params_b -> (the result of phong_shade_backward without vis_b, sun_vis_b and spec_b, the maps' gradients in
+        the order of self._maps, spec_b or None)."""
         shaded = phong_shade_backward(gbuffer, params, center, background, image_b, self._phong_scratch,
                                       center_grad=camera_grad, sh=self.sh, albedo=albedo,
-                                      point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis)
+                                      point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis,
+                                      specular=spec)
+        spec_b = None
+        if spec is not None:
+            shaded, spec_b = shaded[:-1], shaded[-1]
         maps_b = []
         sun_b = None
         if sun_vis is not None:
@@ -1734,7 +1809,7 @@ class DeviceMeshView:
                                                   self.light_shadow_bias, self.light_shadow_softness, sun_b,
                                                   self._phong_scratch, albedo=albedo, channels_b=shaded[0],
                                                   map_b=self._sun.zero_maps_b()[0], light_b=shaded[1])[1][None])
-        return shaded, maps_b
+        return shaded, maps_b, spec_b
 
     def _phong_params(self) -> Tuple[torch.Tensor, torch.Tensor]:
         """(params [6], camera_center [3]) fp64 on the device, uploaded again only when the light, the specular
@@ -1808,11 +1883,13 @@ class DeviceMeshView:
         return camera_gradients(camera, camera_b, self._camera_distorted, center_b)
 
     def render(self, vertices: torch.Tensor, vertex_colors: Optional[torch.Tensor] = None,
-               texture: Optional[torch.Tensor] = None, normal_map: Optional[torch.Tensor] = None) -> torch.Tensor:
+               texture: Optional[torch.Tensor] = None, normal_map: Optional[torch.Tensor] = None,
+               specular_map: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The image [H,W,C] f32 of the mesh at ``vertices`` [V,3]: Gouraud-lit ``vertex_colors`` [V,C] for an untextured
         view; for a textured one the texture shaded by the vertex luminosity, with ``texture`` [Ht,Wt,C] (if given)
         copied into the view's texture first, so that a fit can vary it.  ``normal_map`` [Ht,Wt,3], in a view made with
-        one, is copied into the view's normal map in the same way."""
+        one, is copied into the view's normal map in the same way, and ``specular_map`` [Ht,Wt,2] into its specular
+        map."""
         if normal_map is not None:
             if not self.normal_mapped:
                 raise ValueError("this view has no normal map (DeviceMeshView(..., normal_map=) makes one)")
@@ -1820,6 +1897,13 @@ class DeviceMeshView:
                 raise ValueError(f"normal_map has shape {tuple(normal_map.shape)}, expected "
                                  f"{tuple(self._map_scene.t['texture'].shape)}")
             self._map_scene.t["texture"].copy_(normal_map)
+        if specular_map is not None:
+            if not self.specular_mapped:
+                raise ValueError("this view has no specular map (DeviceMeshView(..., specular_map=) makes one)")
+            if tuple(specular_map.shape) != tuple(self._spec_scene.t["texture"].shape):
+                raise ValueError(f"specular_map has shape {tuple(specular_map.shape)}, expected "
+                                 f"{tuple(self._spec_scene.t['texture'].shape)}")
+            self._spec_scene.t["texture"].copy_(specular_map)
         if self.textured:
             if vertex_colors is not None:
                 raise ValueError("a textured view takes no vertex_colors (its colour is the shaded texture)")
@@ -1880,8 +1964,8 @@ class DeviceMeshView:
         # projection's adjoint
         vertices, _, _, fwd, params, center, vis, sun_vis = self._saved
         nc = self.scene.nb_colors
-        shaded, maps_b = self._shade_backward(fwd["image"], params, center, self.scene.t["background_color"], image_b,
-                                              camera_grad, None, vis, sun_vis)
+        shaded, maps_b, _ = self._shade_backward(fwd["image"], params, center, self.scene.t["background_color"],
+                                                 image_b, camera_grad, None, vis, sun_vis)
         lights_b = None
         if self.point_lights is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
@@ -1934,10 +2018,19 @@ class DeviceMeshView:
             m["depths"].copy_(depths)
             m["edgeflags"].copy_(a["edgeflags"])
             scenes.append(self._map_scene)
+        if self.specular_mapped:
+            # the specular map's raster, last, which shares the geometry too
+            s = self._spec_scene.t
+            s["ij"].copy_(ij)
+            s["depths"].copy_(depths)
+            s["edgeflags"].copy_(a["edgeflags"])
+            scenes.append(self._spec_scene)
         params, center = self._phong_params()
         fwds = self._render_with_maps(scenes, vertices, params)
         gbuffer = normal_map(fwds[1]["image"], fwds[2]["image"]) if self.normal_mapped else fwds[1]["image"]
-        image, vis, sun_vis = self._shade(gbuffer, params, center, self._phong_background, albedo=fwds[0]["image"])
+        spec = fwds[-1]["image"] if self.specular_mapped else None
+        image, vis, sun_vis = self._shade(gbuffer, params, center, self._phong_background, albedo=fwds[0]["image"],
+                                          spec=spec)
         self._gbuffer = gbuffer
         self._saved = (vertices, None, normals, fwds, params, center, vis, sun_vis)
         return image
@@ -1949,10 +2042,13 @@ class DeviceMeshView:
         # are summed before the projection's adjoint.  The albedo raster's shade_b is not used: its shade is constant
         # with a normal map, the perturbation's adjoint first takes the 7-channel channels_b to the 13-channel
         # G-buffer's and the map raster's image gradients; the three rasters' adjoint is one call, the tangent slices
-        # of colors_b go through the tangent frame's adjoint into vertices_b and uv_b, and the ij_b and uv_b summed
+        # of colors_b go through the tangent frame's adjoint into vertices_b and uv_b, and the ij_b and uv_b summed.
+        # A specular map's raster, last, takes the shading's spec_b in the same adjoint call; its ij_b and uv_b are
+        # summed in too
         vertices, _, _, fwds, params, center, vis, sun_vis = self._saved
-        shaded, maps_b = self._shade_backward(self._gbuffer, params, center, self._phong_background, image_b,
-                                              camera_grad, fwds[0]["image"], vis, sun_vis)
+        spec = fwds[-1]["image"] if self.specular_mapped else None
+        shaded, maps_b, spec_b = self._shade_backward(self._gbuffer, params, center, self._phong_background, image_b,
+                                                      camera_grad, fwds[0]["image"], vis, sun_vis, spec)
         lights_b = None
         if self.point_lights is not None:
             shaded, lights_b = shaded[:-1], shaded[-1]
@@ -1962,6 +2058,9 @@ class DeviceMeshView:
             image_bs[1], map_image_b = normal_map_backward(fwds[1]["image"], fwds[2]["image"], channels_b)
             scenes.append(self._map_scene)
             image_bs.append(map_image_b)
+        if self.specular_mapped:
+            scenes.append(self._spec_scene)
+            image_bs.append(spec_b)
         grads = self._render_b_with_maps(scenes, fwds, image_bs, maps_b)
         ga, gg = grads[:2]
         colors_b = gg["colors_b"]
@@ -1974,12 +2073,17 @@ class DeviceMeshView:
         ij_b = ga["ij_b"] + gg["ij_b"]
         if self.normal_mapped:
             ij_b = ij_b + grads[2]["ij_b"]
+        if self.specular_mapped:
+            ij_b = ij_b + grads[-1]["ij_b"]
+            uv_b = uv_b + grads[-1]["uv_b"]
         self._maps_backward(vertices, params, vertices_b, params_b, lights_b)
         _, camera_b = self._project_backward(vertices, ij_b, None, vertices_b, reference_transpose, camera_grad)
         out = {"vertices_b": vertices_b, "texture_b": ga["texture_b"], "uv_b": uv_b, "light_b": params_b[:4],
                "specular_b": params_b[4:]}
         if self.normal_mapped:
             out["normal_map_b"] = grads[2]["texture_b"]
+        if self.specular_mapped:
+            out["specular_map_b"] = grads[-1]["texture_b"]
         if camera_grad:
             out.update(self._camera_result(camera_b, shaded[2]))
         if self.sh is not None:
@@ -2016,7 +2120,8 @@ class DeviceMeshView:
         e_b) for a Phong view, sh_b for a view with an environment and point_lights_b for a view with point lights;
         for a textured view
         dict(vertices_b, texture_b [Ht,Wt,C] f32, uv_b [Nuv,2] f32, light_b), plus specular_b for a textured Phong
-        view (and normal_map_b [Ht,Wt,3] f32 for a normal-mapped one): the luminosity's adjoint ``shade_b`` goes
+        view (and normal_map_b [Ht,Wt,3] f32 for a normal-mapped one, specular_map_b [Ht,Wt,2] f32 for one with a
+        specular map): the luminosity's adjoint ``shade_b`` goes
         through the luminosity and normal adjoints, ``ij_b`` through the projection's.  With ``camera_grad`` the dict
         also holds extrinsic_b, intrinsic_b and distortion_b (see the class); it refuses ``reference_transpose``."""
         if camera_grad and reference_transpose:

@@ -29,16 +29,20 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
                            camera or its centre [3], background [C], sh [9] | [9,C] | None, albedo [H,W,C] | None)
                            -> image [H,W,C] fp32, the per-pixel shading of a G-buffer; a centre tensor and sh receive
                            their gradients.  With a separate albedo the G-buffer is [H,W,7] and the albedo gets one;
-                           point_lights [L, 3 + S] | None get theirs
+                           point_lights [L, 3 + S] | None get theirs; the specular map's raster [H,W,2] | None (with
+                           the albedo) gives the per-pixel ks and e, and receives its gradient
     RenderMeshPhongTexturedFunc  (ij, uv, texture, channels [V,7], depths, edgeflags, albedo scene, G-buffer scene,
                            sigma) -> (albedo [H,W,C], G-buffer [H,W,7]): the two rasters of a textured Phong render
                            in one forward call and one adjoint call; gradients to ij, uv, texture and channels.  With
                            a normal map [Ht,Wt,3] and its scene, channels are [V,13] and a third raster, the map's
-                           [H,W,3], is rendered in the same calls; the map receives its gradient
+                           [H,W,3], is rendered in the same calls; the map receives its gradient.  With a specular map
+                           [Ht,Wt,2] and its scene, one more raster, the map's [H,W,2], is rendered last in the same
+                           calls; the map receives its gradient
     RenderShadowedPhongFunc  (ij, uv | None, texture | None, channels, depths, edgeflags, vertices, point_lights,
                            albedo scene | None, G-buffer scene, ShadowCubes, sigma) -> ([albedo,] G-buffer, cube maps
                            [6L,M,M]): a Phong render's raster(s) and the lights' cube shadow maps in one forward call
-                           and one adjoint call; the maps' share reaches the vertices and the lights' positions
+                           and one adjoint call; the maps' share reaches the vertices and the lights' positions.  A
+                           textured render's normal map and specular map add their rasters as above
     ShadowVisibilityFunc   (G-buffer, point_lights, maps, bias, softness, albedo | None) -> visibility [H,W,L]; the
                            G-buffer, the maps and the lights' positions receive their gradients
     SunVisibilityFunc      (G-buffer, light_directional [3], map [M,M], bounds, bias, softness, albedo | None) ->
@@ -334,7 +338,8 @@ class RenderMeshPhongTexturedFunc(torch.autograd.Function):
     textured with a shade of 1 over a zero background, the G-buffer scene untextured with 7 channels over a zero
     background; both share ij, depths and edge flags.  The forward is one ``render_views`` call and the adjoint one
     ``render_b_views`` call; the two ij gradients are summed.  Same snapshot / replay rule as ``RenderMesh2DFunc``,
-    over both slots: a backward right after its forward replays nothing."""
+    over both slots: a backward right after its forward replays nothing.  The rasters are [albedo, G-buffer, normal
+    map's (with one), specular map's (with one)]."""
 
     NAMES = ("ij", "uv", "shade", "texture")
 
@@ -342,38 +347,43 @@ class RenderMeshPhongTexturedFunc(torch.autograd.Function):
     def forward(ctx: Any, ij: torch.Tensor, uv: torch.Tensor, texture: torch.Tensor,  # type: ignore
                 channels: torch.Tensor, depths: torch.Tensor, edgeflags: torch.Tensor, albedo_scene: DeviceScene,
                 gbuffer_scene: DeviceScene, sigma: float = 1.0, normal_map: Optional[torch.Tensor] = None,
-                map_scene: Optional[DeviceScene] = None):
-        if (normal_map is None) != (map_scene is None):
-            raise ValueError("a normal map comes with its scene")
+                map_scene: Optional[DeviceScene] = None, specular_map: Optional[torch.Tensor] = None,
+                spec_scene: Optional[DeviceScene] = None):
+        if (normal_map is None) != (map_scene is None) or (specular_map is None) != (spec_scene is None):
+            raise ValueError("a normal map or a specular map comes with its scene")
         check_scene_inputs(albedo_scene, uv=uv, texture=texture)
         check_scene_inputs(gbuffer_scene, colors=channels)
         scenes = [albedo_scene, gbuffer_scene]
-        if map_scene is not None:
-            check_scene_inputs(map_scene, uv=uv, texture=normal_map)
-            scenes.append(map_scene)
+        for m, sc in ((normal_map, map_scene), (specular_map, spec_scene)):
+            if sc is not None:
+                check_scene_inputs(sc, uv=uv, texture=m)
+                scenes.append(sc)
         inputs = (ij.detach(), uv.detach(), texture.detach(), channels.detach(), depths.detach(), edgeflags,
-                  normal_map.detach() if normal_map is not None else None)
+                  normal_map.detach() if normal_map is not None else None,
+                  specular_map.detach() if specular_map is not None else None)
         RenderMeshPhongTexturedFunc._update(scenes, *inputs)
         fwds = default_renderer(albedo_scene.device.index).render_views(scenes, sigma)
         ctx.scenes, ctx.sigma, ctx.fwds = scenes, float(sigma), fwds
         ctx.in_dtypes = (ij.dtype, uv.dtype, texture.dtype, channels.dtype,
-                         normal_map.dtype if normal_map is not None else None)
+                         normal_map.dtype if normal_map is not None else None,
+                         specular_map.dtype if specular_map is not None else None)
         ctx.save_for_backward(*(t.clone() if t is not None else None for t in inputs))
         # the caller gets its own tensors: the framebuffers of ctx.fwds may be re-rendered into by backward
         return tuple(f["image"].clone() for f in fwds)
 
     @staticmethod
-    def _update(scenes, ij, uv, texture, channels, depths, edgeflags, normal_map) -> None:
+    def _update(scenes, ij, uv, texture, channels, depths, edgeflags, normal_map, specular_map) -> None:
         scenes[0].update(ij=ij, uv=uv, texture=texture, depths=depths, edgeflags=edgeflags)
         scenes[1].update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
-        if len(scenes) > 2:
-            scenes[2].update(ij=ij, uv=uv, texture=normal_map, depths=depths, edgeflags=edgeflags)
+        for sc, m in zip(scenes[2:], [t for t in (normal_map, specular_map) if t is not None]):
+            sc.update(ij=ij, uv=uv, texture=m, depths=depths, edgeflags=edgeflags)
 
     @staticmethod
     def backward(ctx: Any, *image_bs):  # type: ignore
-        needs = ctx.needs_input_grad[:4] + ctx.needs_input_grad[9:10]
+        ng = ctx.needs_input_grad
+        needs = ng[:4] + ng[9:10] + ng[11:12]
         if not any(needs):
-            return (None,) * 11
+            return (None,) * 13
         scenes = ctx.scenes
         renderer = default_renderer(scenes[0].device.index)
         # the shared scenes may hold another node's inputs by now
@@ -381,19 +391,21 @@ class RenderMeshPhongTexturedFunc(torch.autograd.Function):
         if any(f["generation"] != renderer.generation(f["slot"]) for f in ctx.fwds):
             ctx.fwds = renderer.render_views(scenes, ctx.sigma, out=ctx.fwds)
         names = RenderMeshPhongTexturedFunc.NAMES
+        ij_d, uv_d, tex_d, ch_d, nm_d, sm_d = ctx.in_dtypes
+        # the map rasters and which of normal_map (4) and specular_map (5) each one's texture_b goes to
+        maps = [k for k, d in ((4, nm_d), (5, sm_d)) if d is not None]
         grads = [requested_grads(scenes[0], names, (needs[0], needs[1], False, needs[2])), scenes[1].zero_grads()]
-        if len(scenes) > 2:
-            grads.append(requested_grads(scenes[2], names, (needs[0], needs[1], False, needs[4])))
+        grads += [requested_grads(sc, names, (needs[0], needs[1], False, needs[k])) for sc, k in zip(scenes[2:], maps)]
         renderer.render_b_views(scenes, ctx.sigma, ctx.fwds, [b.contiguous() for b in image_bs], grads=grads)
         ga, gg = grads[:2]
-        ij_d, uv_d, tex_d, ch_d, nm_d = ctx.in_dtypes
         ij_b, uv_b = ga["ij_b"] + gg["ij_b"], ga["uv_b"]
-        if len(scenes) > 2:
-            ij_b, uv_b = ij_b + grads[2]["ij_b"], uv_b + grads[2]["uv_b"]
+        map_b = {}
+        for g, k in zip(grads[2:], maps):
+            ij_b, uv_b = ij_b + g["ij_b"], uv_b + g["uv_b"]
+            map_b[k] = g["texture_b"].to(nm_d if k == 4 else sm_d) if needs[k] else None
         return (ij_b.to(ij_d) if needs[0] else None, uv_b.to(uv_d) if needs[1] else None,
                 ga["texture_b"].to(tex_d) if needs[2] else None, gg["colors_b"].to(ch_d) if needs[3] else None,
-                None, None, None, None, None,
-                grads[2]["texture_b"].to(nm_d) if len(scenes) > 2 and needs[4] else None, None)
+                None, None, None, None, None, map_b.get(4), None, map_b.get(5), None)
 
 
 class PoseFunc(torch.autograd.Function):
@@ -471,14 +483,16 @@ class PhongShadeFunc(torch.autograd.Function):
     the centre [3] as a tensor), background [C], sh, albedo) -> image [H,W,C] fp32.  Backward returns the gradients of
     the channels, of each light and specular parameter and of a centre tensor that needs one, in its dtype; the
     parameter and centre gradients are summed over the pixels in a fixed order.  With ``albedo`` [H,W,C] (a textured
-    mesh's albedo raster) the channels are [H,W,7] = (normal, position, coverage) and the albedo gets its gradient."""
+    mesh's albedo raster) the channels are [H,W,7] = (normal, position, coverage) and the albedo gets its gradient.
+    ``specular_raster`` [H,W,2] (with the albedo) is the specular map's raster (K, E), which gives every specular term
+    aks = ks K and e(p) = e E / a (the model in include/deodr_b200.h), and gets its gradient."""
 
     @staticmethod
     def forward(ctx: Any, channels: torch.Tensor, light_directional: Optional[torch.Tensor],  # type: ignore
                 light_ambient, specular, shininess, camera: CameraParams, background,
                 sh: Optional[torch.Tensor] = None, albedo: Optional[torch.Tensor] = None,
                 point_lights: Optional[torch.Tensor] = None, visibility: Optional[torch.Tensor] = None,
-                sun_visibility: Optional[torch.Tensor] = None):
+                sun_visibility: Optional[torch.Tensor] = None, specular_raster: Optional[torch.Tensor] = None):
         dev = channels.device
         scalars = [x if isinstance(x, torch.Tensor) else torch.tensor(float(x), dtype=torch.float64, device=dev)
                    for x in (light_ambient, specular, shininess)]
@@ -499,9 +513,11 @@ class PhongShadeFunc(torch.autograd.Function):
         pl = _f64(point_lights) if point_lights is not None else None
         vis = visibility.detach().to(torch.float32).contiguous() if visibility is not None else None
         sun = sun_visibility.detach().to(torch.float32).contiguous() if sun_visibility is not None else None
+        spec = specular_raster.detach().to(torch.float32).contiguous() if specular_raster is not None else None
         image = phong_shade(ch, params, center, bg, sh=shd, albedo=alb, point_lights=pl, visibility=vis,
-                            sun_visibility=sun)
-        ctx.save_for_backward(ch, params, center, bg.to(dev, torch.float32), shd, alb, pl, vis, sun)
+                            sun_visibility=sun, specular=spec)
+        ctx.save_for_backward(ch, params, center, bg.to(dev, torch.float32), shd, alb, pl, vis, sun, spec)
+        ctx.spec_dtype = specular_raster.dtype if specular_raster is not None else None
         ctx.vis_dtype = visibility.dtype if visibility is not None else None
         ctx.sun_dtype = sun_visibility.dtype if sun_visibility is not None else None
         ctx.lights_dtype = point_lights.dtype if point_lights is not None else None
@@ -514,11 +530,15 @@ class PhongShadeFunc(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx: Any, image_b: torch.Tensor):  # type: ignore
-        ch, params, center, bg, shd, alb, pl, vis, sun = ctx.saved_tensors
+        ch, params, center, bg, shd, alb, pl, vis, sun, spec = ctx.saved_tensors
         needs = ctx.needs_input_grad
         center_grad = ctx.center_is_input and needs[5]
         shaded = phong_shade_backward(ch, params, center, bg, image_b, _scratch_of(ch.device), center_grad=center_grad,
-                                      sh=shd, albedo=alb, point_lights=pl, visibility=vis, sun_visibility=sun)
+                                      sh=shd, albedo=alb, point_lights=pl, visibility=vis, sun_visibility=sun,
+                                      specular=spec)
+        spec_b = None
+        if spec is not None:
+            shaded, spec_b = shaded[:-1], shaded[-1]
         sun_b = None
         if sun is not None:
             shaded, sun_b = shaded[:-1], shaded[-1]
@@ -544,6 +564,7 @@ class PhongShadeFunc(torch.autograd.Function):
         out.append(lights_b.to(ctx.lights_dtype) if lights_b is not None and needs[9] else None)
         out.append(vis_b.to(ctx.vis_dtype) if vis_b is not None and needs[10] else None)
         out.append(sun_b.to(ctx.sun_dtype) if sun_b is not None and needs[11] else None)
+        out.append(spec_b.to(ctx.spec_dtype) if spec_b is not None and needs[12] else None)
         return tuple(out)
 
 
@@ -566,7 +587,8 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
                 point_lights: Optional[torch.Tensor], albedo_scene: Optional[DeviceScene], gbuffer_scene: DeviceScene,
                 cubes: Optional[ShadowCubes], sigma: float = 1.0, light_directional: Optional[torch.Tensor] = None,
                 sun: Optional[SunShadowMap] = None, normal_map: Optional[torch.Tensor] = None,
-                map_scene: Optional[DeviceScene] = None):
+                map_scene: Optional[DeviceScene] = None, specular_map: Optional[torch.Tensor] = None,
+                spec_scene: Optional[DeviceScene] = None):
         textured = albedo_scene is not None
         if textured:
             check_scene_inputs(albedo_scene, uv=uv, texture=texture)
@@ -578,14 +600,22 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
             raise ValueError("a normal map comes with its scene, in a textured render")
         if mapped:
             check_scene_inputs(map_scene, uv=uv, texture=normal_map)
+        spec_mapped = spec_scene is not None
+        if (specular_map is None) != (not spec_mapped) or (spec_mapped and not textured):
+            raise ValueError("a specular map comes with its scene, in a textured render")
+        if spec_mapped:
+            check_scene_inputs(spec_scene, uv=uv, texture=specular_map)
         inputs = (ij.detach(), uv.detach() if textured else None, texture.detach() if textured else None,
                   channels.detach(), depths.detach(), edgeflags, _f64(vertices.detach()),
                   _f64(point_lights.detach()) if cubes is not None else None,
                   _f64(light_directional.detach()).reshape(3).contiguous() if sun is not None else None,
-                  normal_map.detach() if mapped else None)
-        # the rasters: [albedo,] G-buffer[, normal map]
-        ctx.scenes = ([albedo_scene] if textured else []) + [gbuffer_scene] + ([map_scene] if mapped else [])
+                  normal_map.detach() if mapped else None, specular_map.detach() if spec_mapped else None)
+        # the rasters: [albedo,] G-buffer[, normal map][, specular map]; mi and si index the map rasters
+        ctx.scenes = ([albedo_scene] if textured else []) + [gbuffer_scene] + ([map_scene] if mapped else []) + \
+            ([spec_scene] if spec_mapped else [])
         ctx.gi = 1 if textured else 0
+        ctx.mi = 2 if mapped else None
+        ctx.si = len(ctx.scenes) - 1 if spec_mapped else None
         ctx.maps = [m for m in (cubes, sun) if m is not None]
         ctx.cubes, ctx.sun, ctx.sigma, ctx.textured, ctx.mapped = cubes, sun, float(sigma), textured, mapped
         renderer = default_renderer(gbuffer_scene.device.index)
@@ -593,7 +623,7 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
         ctx.in_dtypes = (ij.dtype, uv.dtype if textured else None, texture.dtype if textured else None, channels.dtype,
                          vertices.dtype, point_lights.dtype if cubes is not None else None,
                          light_directional.dtype if sun is not None else None,
-                         normal_map.dtype if mapped else None)
+                         normal_map.dtype if mapped else None, specular_map.dtype if spec_mapped else None)
         ctx.save_for_backward(*(t.clone() if t is not None else None for t in inputs))
         rasters = tuple(f["image"].clone() for f in ctx.fwds[:len(ctx.scenes)])
         return rasters + ((cubes.maps.clone(),) if cubes is not None else ()) + \
@@ -612,8 +642,10 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
         if ctx.textured:
             ctx.scenes[0].update(ij=ij, uv=uv, texture=texture, depths=depths, edgeflags=edgeflags)
         ctx.scenes[ctx.gi].update(ij=ij, colors=channels, depths=depths, edgeflags=edgeflags)
-        if ctx.mapped:
-            ctx.scenes[2].update(ij=ij, uv=uv, texture=inputs[9], depths=depths, edgeflags=edgeflags)
+        if ctx.mi is not None:
+            ctx.scenes[ctx.mi].update(ij=ij, uv=uv, texture=inputs[9], depths=depths, edgeflags=edgeflags)
+        if ctx.si is not None:
+            ctx.scenes[ctx.si].update(ij=ij, uv=uv, texture=inputs[10], depths=depths, edgeflags=edgeflags)
         RenderShadowedPhongFunc._prepare(ctx, inputs)
 
     @staticmethod
@@ -627,8 +659,8 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx: Any, *grads):  # type: ignore
         needs = ctx.needs_input_grad
-        if not any(needs[:8]) and not needs[12] and not needs[14]:
-            return (None,) * 16
+        if not any(needs[:8]) and not needs[12] and not needs[14] and not needs[16]:
+            return (None,) * 18
         inputs = ctx.saved_tensors
         renderer = default_renderer(ctx.scenes[ctx.gi].device.index)
         n = len(ctx.scenes)
@@ -640,9 +672,12 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
         if ctx.textured:
             gs = [requested_grads(ctx.scenes[0], RenderShadowedPhongFunc.NAMES, (True, needs[1], False, needs[2])),
                   ctx.scenes[1].zero_grads()]
-            if ctx.mapped:
-                gs.append(requested_grads(ctx.scenes[2], RenderShadowedPhongFunc.NAMES,
+            if ctx.mi is not None:
+                gs.append(requested_grads(ctx.scenes[ctx.mi], RenderShadowedPhongFunc.NAMES,
                                           (True, needs[1], False, needs[14])))
+            if ctx.si is not None:
+                gs.append(requested_grads(ctx.scenes[ctx.si], RenderShadowedPhongFunc.NAMES,
+                                          (True, needs[1], False, needs[16])))
         else:
             gs = [ctx.scenes[0].zero_grads()]
         image_bs = [g.to(torch.float32).contiguous() for g in grads[:n]]
@@ -662,9 +697,12 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
         if ctx.sun is not None:
             _, light_b = sun_project_backward(inputs[6], inputs[8], ctx.sun.bounds, ctx.sun.M, ctx.sun.ij_b[0],
                                               ctx.sun.colors_b.view(-1), scratch, vertices_b=vertices_b)
-        ij_d, uv_d, tex_d, ch_d, v_d, l_d, d_d, nm_d = ctx.in_dtypes
+        ij_d, uv_d, tex_d, ch_d, v_d, l_d, d_d, nm_d, sm_d = ctx.in_dtypes
         ij_b = sum(g["ij_b"] for g in gs)
-        uv_b = gs[0]["uv_b"] + gs[2]["uv_b"] if ctx.mapped else gs[0]["uv_b"]
+        uv_b = gs[0]["uv_b"] if ctx.textured else None
+        for i in (ctx.mi, ctx.si):
+            if i is not None:
+                uv_b = uv_b + gs[i]["uv_b"]
         return (ij_b.to(ij_d) if needs[0] else None,
                 uv_b.to(uv_d) if ctx.textured and needs[1] else None,
                 gs[0]["texture_b"].to(tex_d) if ctx.textured and needs[2] else None,
@@ -672,7 +710,8 @@ class RenderShadowedPhongFunc(torch.autograd.Function):
                 vertices_b.to(v_d) if needs[6] else None,
                 lights_b.to(l_d) if lights_b is not None and needs[7] else None,
                 None, None, None, None, light_b.to(d_d) if light_b is not None and needs[12] else None, None,
-                gs[2]["texture_b"].to(nm_d) if ctx.mapped and needs[14] else None, None)
+                gs[ctx.mi]["texture_b"].to(nm_d) if ctx.mi is not None and needs[14] else None, None,
+                gs[ctx.si]["texture_b"].to(sm_d) if ctx.si is not None and needs[16] else None, None)
 
 
 class ShadowVisibilityFunc(torch.autograd.Function):
@@ -880,10 +919,14 @@ class ColoredTriMeshPytorch:
 
     ``normal_map`` [Ht,Wt,3] (a textured mesh's, with the texture's Ht and Wt; a tensor that may require grad, or an
     array) is a tangent-space normal map, read by ``Scene3DPytorch(shading="phong_textured")`` (the model in
-    include/deodr_b200.h); the attribute may be reassigned between renders."""
+    include/deodr_b200.h); the attribute may be reassigned between renders.
+
+    ``specular_map`` [Ht,Wt,2] (a textured mesh's, likewise) is a specular map whose texel (ks_t, e_t) multiplies the
+    scene's specular strength and shininess in a ``phong_textured`` render (the model in include/deodr_b200.h); a tensor
+    that may require grad, or an array, and the attribute may be reassigned between renders."""
 
     def __init__(self, faces, vertices, clockwise: bool = False, colors=None, device=None, faces_uv=None, uv=None,
-                 texture=None, normal_map=None):
+                 texture=None, normal_map=None, specular_map=None):
         self.device = _device(device if device is not None else
                               (vertices.device if isinstance(vertices, torch.Tensor) else None))
         self.faces = np.ascontiguousarray(np.asarray(faces), dtype=np.int64)
@@ -919,6 +962,14 @@ class ColoredTriMeshPytorch:
             if tuple(self.normal_map.shape) != tuple(self.texture.shape[:2]) + (3,):
                 raise ValueError(f"normal_map must be [Ht,Wt,3] with the texture's Ht and Wt = "
                                  f"{tuple(self.texture.shape[:2])}; got {tuple(self.normal_map.shape)}")
+        self.specular_map = None
+        if specular_map is not None:
+            if not self.textured:
+                raise ValueError("a specular map is addressed by the uv: it needs a textured mesh")
+            self.specular_map = self._tensor(specular_map)
+            if tuple(self.specular_map.shape) != tuple(self.texture.shape[:2]) + (2,):
+                raise ValueError(f"specular_map must be [Ht,Wt,2] with the texture's Ht and Wt = "
+                                 f"{tuple(self.texture.shape[:2])}; got {tuple(self.specular_map.shape)}")
 
     @property
     def tangents(self) -> VertexTangents:
@@ -988,7 +1039,9 @@ class Scene3DPytorch:
     :class:`RenderMeshPhongTexturedFunc` node and shaded by :class:`PhongShadeFunc` with the albedo apart; grey and
     coloured environments apply.  A mesh with a ``normal_map`` adds its tangent frames (:class:`VertexTangentsFunc`)
     to the G-buffer and the map's raster to the same node, and :class:`NormalMapFunc` perturbs the G-buffer's normal
-    before the shading and the shadows read it; the map, the uv and the vertices receive their gradients.
+    before the shading and the shadows read it; the map, the uv and the vertices receive their gradients.  A mesh with
+    a ``specular_map`` adds the map's raster to the same node, and :class:`PhongShadeFunc` reads it per pixel; the map
+    receives its gradient.
 
     ``set_point_lights`` adds point lights near the mesh in every shading; a table that requires grad receives its
     gradient, and the vertices receive the lights' share through their normals and their positions.  A flash is a
@@ -1148,13 +1201,13 @@ class Scene3DPytorch:
         return self._phong_scenes[key]
 
     def _albedo_scene(self, camera: CameraPytorch, uv: torch.Tensor, texture: torch.Tensor,
-                      normal_map: bool = False) -> DeviceScene:
-        """The cached albedo raster of a textured mesh for ``camera`` (with ``normal_map``, the normal map's raster, its
-        texture the map): all triangles textured and shaded, a shade of 1 at every vertex (set here once), colours zero,
-        zero background."""
+                      kind: str = "albedo") -> DeviceScene:
+        """The cached albedo raster of a textured mesh for ``camera`` (with ``kind`` "normal_map" or "specular_map", that
+        map's raster, its texture the map): all triangles textured and shaded, a shade of 1 at every vertex (set here
+        once), colours zero, zero background."""
         from ..scenes import SceneArrays
 
-        key = (camera.height, camera.width, tuple(texture.shape), uv.shape[0], normal_map)
+        key = (camera.height, camera.width, tuple(texture.shape), uv.shape[0], kind)
         if key not in self._albedo_scenes:
             m = self.mesh
             T, V, nc = m.nb_faces, m.nb_vertices, texture.shape[2]
@@ -1189,12 +1242,21 @@ class Scene3DPytorch:
                 raise ValueError(f"normal_map must be [Ht,Wt,3] with the texture's Ht and Wt = "
                                  f"{tuple(texture.shape[:2])}; got {tuple(nmap.shape)}")
             channels = torch.cat((channels, vertex_tangents_autograd(m.vertices, uv, m.tangents)), dim=1)
-            map_scene = self._albedo_scene(camera, uv, nmap, normal_map=True)
+            map_scene = self._albedo_scene(camera, uv, nmap, kind="normal_map")
+        smap = spec_scene = None
+        if m.specular_map is not None:
+            # the specular map's raster, after the others
+            smap = m._tensor(m.specular_map)
+            if tuple(smap.shape) != tuple(texture.shape[:2]) + (2,):
+                raise ValueError(f"specular_map must be [Ht,Wt,2] with the texture's Ht and Wt = "
+                                 f"{tuple(texture.shape[:2])}; got {tuple(smap.shape)}")
+            spec_scene = self._albedo_scene(camera, uv, smap, kind="specular_map")
+        rasters = 2 + (nmap is not None) + (smap is not None)
         vis = sun = None
         if self.shadow_map_size or self.light_shadow_map_size:
             out = self._render_shadowed(ij, uv, texture, channels, depths, self._albedo_scene(camera, uv, texture),
-                                        self._phong_scene(camera, 0, nmap is not None), nmap, map_scene)
-            rasters = 3 if nmap is not None else 2
+                                        self._phong_scene(camera, 0, nmap is not None), nmap, map_scene, smap,
+                                        spec_scene)
             albedo, gbuffer = out[:2]
             if nmap is not None:
                 gbuffer = normal_map_autograd(gbuffer, out[2])
@@ -1203,13 +1265,14 @@ class Scene3DPytorch:
             out = render_mesh_phong_textured(ij, uv, texture, channels, depths, self._edgeflags(ij),
                                              self._albedo_scene(camera, uv, texture),
                                              self._phong_scene(camera, 0, nmap is not None), self.sigma, nmap,
-                                             map_scene)
+                                             map_scene, smap, spec_scene)
             albedo, gbuffer = out[:2]
             if nmap is not None:
                 gbuffer = normal_map_autograd(gbuffer, out[2])
+        spec = out[rasters - 1] if smap is not None else None
         return phong_shade_autograd(gbuffer, self.light_directional, self.light_ambient, self.specular,
                                     self.shininess, camera.center() if camera.is_tensor else camera,
-                                    self.background_color, self.light_sh, albedo, self.point_lights, vis, sun)
+                                    self.background_color, self.light_sh, albedo, self.point_lights, vis, sun, spec)
 
     def _render_phong(self, camera: CameraPytorch) -> torch.Tensor:
         m = self.mesh
@@ -1238,7 +1301,7 @@ class Scene3DPytorch:
                                     self.light_sh, None, self.point_lights, vis, sun)
 
     def _render_shadowed(self, ij, uv, texture, channels, depths, albedo_scene, gbuffer_scene, normal_map=None,
-                         map_scene=None) -> tuple:
+                         map_scene=None, specular_map=None, spec_scene=None) -> tuple:
         """The rasters and the shadow maps in one :class:`RenderShadowedPhongFunc` node."""
         m = self.mesh
         cubes = self._shadow_cubes() if self.shadow_map_size else None
@@ -1246,7 +1309,7 @@ class Scene3DPytorch:
         return render_shadowed_phong(ij, uv, texture, channels, depths, self._edgeflags(ij), m.vertices,
                                      self.point_lights if cubes is not None else None, albedo_scene, gbuffer_scene,
                                      cubes, self.sigma, self.light_directional if sun is not None else None, sun,
-                                     normal_map, map_scene)
+                                     normal_map, map_scene, specular_map, spec_scene)
 
     def _visibilities(self, gbuffer, maps, albedo) -> tuple:
         """(the point lights' visibility or None, the directional light's or None) from the node's maps."""

@@ -867,6 +867,54 @@ int deodr_b200_normal_map(const float *gbuffer, const float *map, int H, int W, 
 int deodr_b200_normal_map_b(const float *gbuffer, const float *map, int H, int W, const float *out_b,
                             float *gbuffer_b, float *map_b, void *stream);
 
+/* ---- specular maps (textured Phong) -------------------------------------------------------------------------------
+ * A specular map S [Ht, Wt, 2] fp32 has the albedo texture's Ht and Wt and is addressed by the same uv / faces_uv.  It
+ * follows the glTF convention, factor x texture: texel (ks_t, e_t) multiplies the view's ks = params[4] and e =
+ * params[5], so a map of ones is the view without a map, and ks and e keep their meaning and their gradient.  The map
+ * is rasterised like the albedo (shade 1, zero background, 2 channels, the view's geometry and sigma), which gives per
+ * pixel (K, E) = a x (sample of S), a the G-buffer's coverage.  Per pixel, in the Phong form with a separate albedo:
+ *
+ *   aks(p) = ks * K          in place of a * ks, in spec and in every point light's spec_j
+ *   e(p)   = e * (E / a)     in place of e (read only where a != 0: every specular term is 0 at a = 0)
+ *
+ * Nothing else changes: the diffuse, ambient and environment terms, the point lights' diffuse terms and the
+ * visibilities V_j and V multiply as before.  E / a is rounded first, so that a map of ones (E = a) gives e exactly.
+ * Over the background K / a and E / a are the front surface's values; at self-occlusion silhouettes front and back are
+ * mixed, as for the normals.
+ *
+ * Adjoint, with q the gradient of aks(p) and e_b(p) that of e(p), each summed over the main term and the point lights:
+ *
+ *   K_b = q * ks,   ks_b += q * K
+ *   E_b = e_b(p) * e / a,   e_b += e_b(p) * E / a,   a_b -= e_b(p) * e(p) / a
+ *
+ * The a * ks share of a_b of the view without a map is gone: ks reaches the image through K only.  spec_b = (K_b, E_b)
+ * is 0 where a = 0.  params_b stays a fixed-order sum (bit-reproducible, no fp64 atomics); the map raster's gradient
+ * then goes through the rasteriser's adjoint to the map's texels, the uv and ij.
+ *
+ * Limitations: grey specular only (one ks per texel); bilinear sampling without mip levels; e(p) <= 0 gives what pow
+ * gives, so a fit that can drive e_t or e negative parametrises it itself. */
+
+/* The Phong shading of deodr_b200_phong_shade_sun_shadowed with a separate albedo [H,W,C] and the specular map's
+ * raster spec [H,W,2] = (K, E), both required, an optional environment (sh NULL with sh_channels 0), optional point
+ * lights (lights NULL with nb_lights 0) with their optional visibility vis [H,W,L], and an optional sun visibility
+ * sun_vis [H,W] (NULL: the directional light is unshadowed).  DeodrPhongIO is read as by
+ * deodr_b200_phong_shade_albedo; its layout is unchanged.  The refusals of the calls it extends, before any launch:
+ * DEODR_B200_EINVAL for a NULL io, buffer, albedo or spec, bad sizes or offsets (off_albedo must be -1), a NULL sh with
+ * sh_channels != 0, or a NULL lights with nb_lights != 0 or a vis; DEODR_B200_EUNSUPPORTED for bad channel or light
+ * counts.  No host synchronisation. */
+int deodr_b200_phong_shade_specular_map(const DeodrPhongIO *io, const float *albedo, const float *spec,
+                                        const double *sh, int sh_channels, const double *lights, int nb_lights,
+                                        int light_channels, const float *vis, const float *sun_vis, void *stream);
+/* Its adjoint from io->image_b: channels_b [H,W,7], albedo_b [H,W,C], spec_b [H,W,2], params_b and camera_center_b
+ * (when given) overwritten, and with the optional inputs sh_b, lights_b, vis_b and sun_vis_b as the calls it extends
+ * write them (each may be NULL without its input).  Same refusals, plus DEODR_B200_EINVAL for a NULL image_b,
+ * channels_b, params_b, albedo_b, spec_b or scratch, or a NULL gradient of a given optional input. */
+int deodr_b200_phong_shade_specular_map_b(const DeodrPhongIO *io, const float *albedo, const float *spec,
+                                          const double *sh, int sh_channels, const double *lights, int nb_lights,
+                                          int light_channels, const float *vis, const float *sun_vis,
+                                          float *albedo_b, float *spec_b, double *sh_b, double *lights_b,
+                                          float *vis_b, float *sun_vis_b, double *scratch, void *stream);
+
 /* One parameter vector of a heavy-ball update (device pointers, `size` entries each):
  *   step = clamp(-grad * factor, -max_step, max_step)   (max_step = INFINITY: unclamped)
  *   speed = (1 - damping) (speed * inertia + (1 - inertia) step);  value += speed
