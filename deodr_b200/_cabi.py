@@ -385,6 +385,12 @@ SYMBOLS = [
     ("deodr_b200_phong_shade_specular_map_b", C.c_int,
      [C.POINTER(PhongIO), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_pbr_shade", C.c_int,
+     [C.POINTER(PhongIO), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+      C.c_void_p, C.c_void_p]),
+    ("deodr_b200_pbr_shade_b", C.c_int,
+     [C.POINTER(PhongIO), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("deodr_b200_vertex_tangents", C.c_int,
      [C.POINTER(MeshTopology), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("deodr_b200_vertex_tangents_b", C.c_int,

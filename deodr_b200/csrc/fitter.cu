@@ -612,6 +612,122 @@ __device__ __forceinline__ void point_term_b(const PointTerm &t, const double n[
     }
 }
 
+// ---- metallic-roughness (GGX) shading (the model of include/deodr_b200.h) ----------------------------------------
+
+// The scalars of one light of unit direction w for unit normal n and view v, with k = alpha^2: nl = <n, w>; where
+// nl > 0, nv, nh and vh (clamped at 0), h = normalize(w + v) (0 when w + v = 0), Fs = (1 - vh)^5 and, where k > 0, S
+// = pi D V = k / (Dd^2 Vl Vv), Dd = nh^2 (k - 1) + 1, Vl = nl + ql, ql = sqrt(k + (1 - k) nl^2) (Vv, qv alike).
+// Every other field is 0.  The light's term is E nl [(1 - F)(1 - m) A + a S F] with F = F0 + (1 - F0) Fs.
+struct GgxTerm {
+    double nl, nv, nh, vh, hn, h[3], Dd, ql, qv, Vl, Vv, S, Fs;
+};
+
+__device__ __forceinline__ void ggx_term(const double n[3], const double v[3], const double w[3], double k,
+                                         GgxTerm &t) {
+    t.nl = dot(n, w);
+    t.S = t.Fs = 0.0;
+    if (!(t.nl > 0)) return;
+    double hh[3];
+    for (int j = 0; j < 3; j++) hh[j] = w[j] + v[j];
+    t.hn = sqrt(dot(hh, hh));
+    for (int j = 0; j < 3; j++) t.h[j] = t.hn == 0.0 ? 0.0 : hh[j] / t.hn;
+    const double cv = dot(n, v), ch = dot(n, t.h), cvh = dot(v, t.h);
+    t.nv = cv > 0 ? cv : 0.0;
+    t.nh = ch > 0 ? ch : 0.0;
+    t.vh = cvh > 0 ? cvh : 0.0;
+    const double o = 1.0 - t.vh, o2 = o * o;
+    t.Fs = (o2 * o2) * o;
+    if (!(k > 0)) return;
+    t.Dd = (t.nh * t.nh) * (k - 1.0) + 1.0;
+    t.ql = sqrt(k + (1.0 - k) * (t.nl * t.nl));
+    t.qv = sqrt(k + (1.0 - k) * (t.nv * t.nv));
+    t.Vl = t.nl + t.ql;
+    t.Vv = t.nv + t.qv;
+    t.S = k / ((t.Dd * t.Dd) * (t.Vl * t.Vv));
+}
+
+// The adjoint of ggx_term from nl_b (nl's gradient through the term's factor nl), S_b and Fs_b: adds to n_b, v_b,
+// w_b and k_b.
+__device__ __forceinline__ void ggx_term_b(const GgxTerm &t, const double n[3], const double v[3], const double w[3],
+                                           double k, double nl_b, double S_b, double Fs_b, double n_b[3],
+                                           double v_b[3], double w_b[3], double &k_b) {
+    if (!(t.nl > 0)) return;
+    double nv_b = 0, nh_b = 0;
+    if (k > 0) {
+        const double Sl = t.S / t.Vl, Sv = t.S / t.Vv;
+        k_b += S_b * (1.0 / ((t.Dd * t.Dd) * (t.Vl * t.Vv)) -
+                      ((2.0 * t.S) * (t.nh * t.nh) / t.Dd + Sl * (1.0 - t.nl * t.nl) / (2.0 * t.ql) +
+                       Sv * (1.0 - t.nv * t.nv) / (2.0 * t.qv)));
+        nh_b = -S_b * (4.0 * t.S) * t.nh * (k - 1.0) / t.Dd;
+        nl_b -= S_b * Sl * (1.0 + (1.0 - k) * t.nl / t.ql);
+        nv_b = -S_b * Sv * (1.0 + (1.0 - k) * t.nv / t.qv);
+    }
+    const double o = 1.0 - t.vh, vh_b = -5.0 * Fs_b * ((o * o) * (o * o));
+    double h_b[3] = {0, 0, 0};
+    for (int j = 0; j < 3; j++) {
+        n_b[j] += nl_b * w[j];
+        w_b[j] += nl_b * n[j];
+        if (t.nv > 0) {
+            n_b[j] += nv_b * v[j];
+            v_b[j] += nv_b * n[j];
+        }
+        if (t.nh > 0) {
+            n_b[j] += nh_b * t.h[j];
+            h_b[j] += nh_b * n[j];
+        }
+        if (t.vh > 0) {
+            v_b[j] += vh_b * t.h[j];
+            h_b[j] += vh_b * v[j];
+        }
+    }
+    if (t.hn != 0.0) {
+        double hh_b[3] = {0, 0, 0};
+        normalize_b(t.h, h_b, t.hn, hh_b);  // hh = w + v
+        for (int j = 0; j < 3; j++) {
+            w_b[j] += hh_b[j];
+            v_b[j] += hh_b[j];
+        }
+    }
+}
+
+// One light's shares of the three sums its term is formed from, for a grey factor E (the intensity and visibility
+// with the falloff): t1 = E nl (1 - Fs), t2 = E nl S (1 - Fs) and t3 = E nl S Fs; a channel's term is then
+// (1 - m) A (1 - F0) t1 + a F0 t2 + a t3.  Given u1..u3, the gradients of t1..t3, ggx_sums_b returns E's gradient
+// and calls ggx_term_b with those of nl, S and Fs.
+__device__ __forceinline__ void ggx_sums(const GgxTerm &t, double E, double out[3]) {
+    const double e = t.nl > 0 ? E * t.nl : 0.0, es = e * t.S;
+    out[0] = e * (1.0 - t.Fs);
+    out[1] = es * (1.0 - t.Fs);
+    out[2] = es * t.Fs;
+}
+
+__device__ __forceinline__ double ggx_sums_b(const GgxTerm &t, double E, const double u[3], const double n[3],
+                                             const double v[3], const double w[3], double k, double n_b[3],
+                                             double v_b[3], double w_b[3], double &k_b) {
+    if (!(t.nl > 0)) return 0.0;
+    const double f = (u[0] + u[1] * t.S) * (1.0 - t.Fs) + (u[2] * t.S) * t.Fs;
+    const double e = E * t.nl;
+    ggx_term_b(t, n, v, w, k, E * f, e * (u[1] * (1.0 - t.Fs) + u[2] * t.Fs), e * ((u[2] - u[1]) * t.S - u[0]),
+               n_b, v_b, w_b, k_b);
+    return t.nl * f;
+}
+
+// The material of a covered pixel (a != 0) from the factors mf = params[4] and rf = params[5], and the map raster mr
+// [H,W,2] = (R, M) when given: r = rf (R / a), m = mf (M / a) (R / a and M / a rounded first), k = alpha^2 = r^4.
+struct GgxMaterial {
+    double R, M, r, m, k;  // R, M: R / a and M / a (1 without a map)
+};
+
+__device__ __forceinline__ void ggx_material(const double *prm, double a, const float *mr, long long p,
+                                             GgxMaterial &mt) {
+    mt.R = mr ? (double)mr[2 * p] / a : 1.0;
+    mt.M = mr ? (double)mr[2 * p + 1] / a : 1.0;
+    mt.r = prm[5] * mt.R;
+    mt.m = prm[4] * mt.M;
+    const double r2 = mt.r * mt.r;
+    mt.k = r2 * r2;
+}
+
 // Sums v[0..K) over a grid of (rows) x (G CTAs per row) in a fixed order and writes the totals of row i to
 // out[i K .. i K + K): CTA (i, y) sums its items into the partials [i][k][y]; the last CTA to finish adds them over y
 // in CTA order (the pattern of k_pose_frames_b).  rows K G must not exceed MAX_K * MAX_CTAS.
@@ -907,6 +1023,295 @@ __device__ __forceinline__ float &albedo_b_at(float *pb, const DeodrPhongIO &io,
     return SPLIT ? albedo_b[p * io.C + c] : pb[io.off_albedo + c];
 }
 
+// The GGX form's image of pixel p (k_phong_shade with GGX; the model of include/deodr_b200.h).  Each light adds its
+// ggx_sums into three grey sums (the directional light, grey point lights) or three per channel (coloured point
+// lights, P > 1); the channels expand them where the image is formed.  0 surface terms where a = 0.
+template <int S, int P, bool VIS, bool SUN>
+__device__ __forceinline__ void ggx_shade(const DeodrPhongIO &io, const float *px, long long p, const double *sh,
+                                          const float *albedo, const double *lights, int L, const float *vis,
+                                          const float *sun_vis, const float *mr, float *out) {
+    constexpr int NC = S > P ? S : P, PC = P > 1 ? P : 1;
+    const int C = io.C;
+    const double *prm = io.params;
+    const double a = px[io.off_coverage];
+    if (a == 0.0) {
+        for (int c = 0; c < C; c++) out[c] = (float)((1.0 - a) * (double)io.background[c]);
+        return;
+    }
+    const double N[3] = {px[io.off_normal], px[io.off_normal + 1], px[io.off_normal + 2]};
+    const double nn = sqrt(dot(N, N));
+    double n[3], x[3], v[3];
+    for (int j = 0; j < 3; j++) {
+        n[j] = nn == 0.0 ? 0.0 : N[j] / nn;
+        x[j] = px[io.off_position + j] / a;
+        v[j] = io.camera_center[j] - x[j];
+    }
+    const double dn = sqrt(dot(v, v));
+    for (int j = 0; j < 3; j++) v[j] /= dn;
+    GgxMaterial mt;
+    ggx_material(prm, a, mr, p, mt);
+    double sg[3] = {0, 0, 0}, sc[3][PC], tt[3];
+#pragma unroll
+    for (int c = 0; c < PC; c++) sc[0][c] = sc[1][c] = sc[2][c] = 0;
+    const double l[3] = {prm[0], prm[1], prm[2]};
+    const double ll = sqrt(dot(l, l));
+    if (ll > 0) {
+        const double w[3] = {-l[0] / ll, -l[1] / ll, -l[2] / ll};
+        GgxTerm t;
+        ggx_term(n, v, w, mt.k, t);
+        ggx_sums(t, SUN ? ll * (double)sun_vis[p] : ll, tt);
+        for (int k = 0; k < 3; k++) sg[k] += tt[k];
+    }
+    if constexpr (P > 0)
+        for (int j = 0; j < L; j++) {
+            const double *lj = lights + j * (3 + P);
+            double d[3], w[3];
+            for (int k = 0; k < 3; k++) d[k] = lj[k] - x[k];
+            const double r2 = dot(d, d), r = sqrt(r2);
+            if (!(r > 0)) continue;
+            for (int k = 0; k < 3; k++) w[k] = d[k] / r;
+            GgxTerm t;
+            ggx_term(n, v, w, mt.k, t);
+            double E = (P == 1 ? lj[3] : 1.0) / r2;
+            if constexpr (VIS) E *= (double)vis[p * L + j];
+            ggx_sums(t, E, tt);
+            if (P == 1) {
+                for (int k = 0; k < 3; k++) sg[k] += tt[k];
+            } else {
+#pragma unroll
+                for (int c = 0; c < PC; c++)
+                    for (int k = 0; k < 3; k++) sc[k][c] += lj[3 + c] * tt[k];
+            }
+        }
+    double Y[9];
+    if (S > 0) sh_basis(n, Y);
+    const double kd = 1.0 - mt.m;
+    auto shade = [&](int c) {
+        const double A = albedo[p * C + c], F0 = 0.04 * kd + mt.m * (A / a);
+        const int q = P > 1 ? c : 0;
+        const double s1 = sg[0] + (P > 1 ? sc[0][q] : 0.0), s2 = sg[1] + (P > 1 ? sc[1][q] : 0.0),
+                     s3 = sg[2] + (P > 1 ? sc[2][q] : 0.0);
+        const double amb = S > 0 ? prm[3] + sh_value<(S > 0 ? S : 1)>(sh, S > 1 ? c : 0, Y) : prm[3];
+        return (float)(((kd * A) * ((1.0 - F0) * s1 + amb) + a * (F0 * s2 + s3)) +
+                       (1.0 - a) * (double)io.background[c]);
+    };
+    if (NC > 1) {
+#pragma unroll
+        for (int c = 0; c < NC; c++) out[c] = shade(c);
+    } else {
+        for (int c = 0; c < C; c++) out[c] = shade(c);
+    }
+}
+
+// The adjoint of ggx_shade for pixel p (k_phong_shade_b with GGX): albedo_b, channels_b, mr_b (with mr), vis_b and
+// sun_vis_b written; l_b, ambient_b, mf_b, rf_b (and, CENTER, camera_center_b) added to acc.  A first pass over the
+// channels forms u = the gradients of the three sums (grey: U; per channel: uc), the environment's normal gradient
+// and env_c; a forward pass over the lights forms the sums, a second pass over the channels takes the material's
+// adjoint from them, and the lights' loop then takes each light's adjoint from u (ggx_sums_b).
+template <bool CENTER, int S, int P, bool VIS, bool SUN, int K>
+__device__ __forceinline__ void ggx_shade_b(const DeodrPhongIO &io, long long p, const double *sh,
+                                            const float *albedo, float *albedo_b, const double *lights, int L,
+                                            const float *vis, float *vis_b, const float *sun_vis, float *sun_vis_b,
+                                            const float *mr, float *mr_b, double (&acc)[K]) {
+    constexpr int NC = S > P ? S : P, PC = P > 1 ? P : 1;
+    const int C = io.C;
+    const double *prm = io.params;
+    const float *px = io.channels + p * 7;
+    const float *g = io.image_b + p * C;
+    float *pb = io.channels_b + p * 7;
+    const double a = px[io.off_coverage];
+    if (a == 0.0) {
+        double bg_b = 0;
+        for (int c = 0; c < C; c++) {
+            bg_b += (double)io.background[c] * (double)g[c];
+            albedo_b[p * C + c] = 0.0f;
+        }
+        for (int j = 0; j < 3; j++) pb[io.off_normal + j] = pb[io.off_position + j] = 0.0f;
+        pb[io.off_coverage] = (float)-bg_b;
+        if (mr) mr_b[2 * p] = mr_b[2 * p + 1] = 0.0f;
+        if constexpr (VIS)
+            for (int j = 0; j < L; j++) vis_b[p * L + j] = 0.0f;
+        if constexpr (SUN) sun_vis_b[p] = 0.0f;
+        return;
+    }
+    const double N[3] = {px[io.off_normal], px[io.off_normal + 1], px[io.off_normal + 2]};
+    const double nn = sqrt(dot(N, N));
+    double n[3], x[3], v[3];
+    for (int j = 0; j < 3; j++) {
+        n[j] = nn == 0.0 ? 0.0 : N[j] / nn;
+        x[j] = px[io.off_position + j] / a;
+        v[j] = io.camera_center[j] - x[j];
+    }
+    const double dn = sqrt(dot(v, v));
+    for (int j = 0; j < 3; j++) v[j] /= dn;
+    GgxMaterial mt;
+    ggx_material(prm, a, mr, p, mt);
+    const double kd = 1.0 - mt.m;
+    // u(c): channel c's gradients of the three sums; U = sum_c u(c), the grey lights'.  Coloured lights (P > 1)
+    // form sum_c u(c) I_j[c] in their loop, from u(c) formed again there rather than kept
+    auto u_of = [&](int c, double u[3]) {
+        const double A = albedo[p * C + c], gc = g[c], F0 = 0.04 * kd + mt.m * (A / a);
+        u[0] = gc * (kd * A) * (1.0 - F0);
+        u[1] = gc * (a * F0);
+        u[2] = gc * a;
+    };
+    double U[3] = {0, 0, 0}, env[S > 0 ? S : 1], n_b[3] = {0, 0, 0};
+    {
+        double Y[9], wsh[9];
+        if (S > 0) {
+            sh_basis(n, Y);
+#pragma unroll
+            for (int k = 0; k < 9; k++) wsh[k] = 0;
+            if (S == 1) env[0] = sh_value<1>(sh, 0, Y);
+        }
+        auto pass1 = [&](int c) {
+            double u[3];
+            u_of(c, u);
+            for (int k = 0; k < 3; k++) U[k] += u[k];
+            if constexpr (S > 0) {
+                const double gA = (double)g[c] * (kd * (double)albedo[p * C + c]);
+#pragma unroll
+                for (int k = 0; k < 9; k++) wsh[k] += gA * sh[k * S + (S > 1 ? c : 0)];
+                if (S > 1) env[S > 1 ? c : 0] = sh_value<(S > 0 ? S : 1)>(sh, c, Y);
+            }
+        };
+        if (NC > 1) {
+#pragma unroll
+            for (int c = 0; c < NC; c++) pass1(c);
+        } else {
+            for (int c = 0; c < C; c++) pass1(c);
+        }
+        if (S > 0) sh_grad_add(n, wsh, n_b);
+    }
+    // the sums, a forward pass over the lights: their per-channel values are not live in the adjoint's loop below
+    double sg[3] = {0, 0, 0}, sc[3][PC], tt[3];
+#pragma unroll
+    for (int c = 0; c < PC; c++) sc[0][c] = sc[1][c] = sc[2][c] = 0;
+    const double l[3] = {prm[0], prm[1], prm[2]};
+    const double ll = sqrt(dot(l, l));
+    const double sv = SUN ? (double)sun_vis[p] : 1.0;
+    if (ll > 0) {
+        const double w[3] = {-l[0] / ll, -l[1] / ll, -l[2] / ll};
+        GgxTerm t;
+        ggx_term(n, v, w, mt.k, t);
+        ggx_sums(t, SUN ? ll * sv : ll, tt);
+        for (int k = 0; k < 3; k++) sg[k] += tt[k];
+    }
+    if constexpr (P > 0)
+        for (int j = 0; j < L; j++) {
+            const double *lj = lights + j * (3 + P);
+            double d[3], w[3];
+            for (int k = 0; k < 3; k++) d[k] = lj[k] - x[k];
+            const double r2 = dot(d, d), r = sqrt(r2);
+            if (!(r > 0)) continue;
+            for (int k = 0; k < 3; k++) w[k] = d[k] / r;
+            GgxTerm t;
+            ggx_term(n, v, w, mt.k, t);
+            const double E0 = (P == 1 ? lj[3] : 1.0) / r2;
+            ggx_sums(t, VIS ? E0 * (double)vis[p * L + j] : E0, tt);
+            if (P == 1) {
+                for (int k = 0; k < 3; k++) sg[k] += tt[k];
+            } else {
+#pragma unroll
+                for (int c = 0; c < PC; c++)
+                    for (int k = 0; k < 3; k++) sc[k][c] += lj[3 + c] * tt[k];
+            }
+        }
+    // the material: F0_c = 0.04 kd + m b_c, b_c = A_c / a, kd = 1 - m
+    double kd_b = 0, m_b = 0, a_b = 0;
+    auto pass2 = [&](int c) {
+        const double A = albedo[p * C + c], gc = g[c], b = A / a, F0 = 0.04 * kd + mt.m * b;
+        const int q = P > 1 ? c : 0;
+        const double s1 = sg[0] + (P > 1 ? sc[0][q] : 0.0), s2 = sg[1] + (P > 1 ? sc[1][q] : 0.0),
+                     s3 = sg[2] + (P > 1 ? sc[2][q] : 0.0);
+        const double lum = (1.0 - F0) * s1 + (S > 0 ? prm[3] + env[S > 1 ? c : 0] : prm[3]);
+        const double F0_b = gc * (a * s2 - (kd * A) * s1), b_b = F0_b * mt.m;
+        kd_b += gc * A * lum + 0.04 * F0_b;
+        m_b += F0_b * b;
+        a_b += gc * ((F0 * s2 + s3) - (double)io.background[c]) - b_b * b / a;
+        acc[3] += gc * (kd * A);
+        albedo_b[p * C + c] = (float)(gc * kd * lum + b_b / a);
+    };
+    if (NC > 1) {
+#pragma unroll
+        for (int c = 0; c < NC; c++) pass2(c);
+    } else {
+        for (int c = 0; c < C; c++) pass2(c);
+    }
+    m_b -= kd_b;
+    // the lights' adjoint, each term formed again
+    double v_b[3] = {0, 0, 0}, x_b[3] = {0, 0, 0}, k_b = 0;
+    if (ll > 0) {
+        // E = |l| V, w = -l / |l|
+        const double w[3] = {-l[0] / ll, -l[1] / ll, -l[2] / ll};
+        GgxTerm t;
+        ggx_term(n, v, w, mt.k, t);
+        double w_b[3] = {0, 0, 0};
+        const double E_b = ggx_sums_b(t, SUN ? ll * sv : ll, U, n, v, w, mt.k, n_b, v_b, w_b, k_b);
+        if constexpr (SUN) sun_vis_b[p] = (float)(E_b * ll);
+        const double ll_b = SUN ? E_b * sv : E_b, pr = dot(w, w_b);
+        for (int j = 0; j < 3; j++) acc[j] += -ll_b * w[j] - (w_b[j] - w[j] * pr) / ll;
+    } else if constexpr (SUN) {
+        sun_vis_b[p] = 0.0f;
+    }
+    if constexpr (P > 0)
+        for (int j = 0; j < L; j++) {
+            // E = I V / r^2 (I = 1 for coloured lights: their intensities are in uj), w = d / r, d = p_j - x
+            const double *lj = lights + j * (3 + P);
+            double d[3], w[3], w_b[3] = {0, 0, 0}, d_b[3] = {0, 0, 0};
+            for (int k = 0; k < 3; k++) d[k] = lj[k] - x[k];
+            const double r2 = dot(d, d), r = sqrt(r2);
+            if (!(r > 0)) {
+                if constexpr (VIS) vis_b[p * L + j] = 0.0f;
+                continue;
+            }
+            for (int k = 0; k < 3; k++) w[k] = d[k] / r;
+            GgxTerm t;
+            ggx_term(n, v, w, mt.k, t);
+            const double E0 = (P == 1 ? lj[3] : 1.0) / r2, E = VIS ? E0 * (double)vis[p * L + j] : E0;
+            double uj[3];
+            if (P == 1) {
+                for (int k = 0; k < 3; k++) uj[k] = U[k];
+            } else {
+                for (int k = 0; k < 3; k++) uj[k] = 0;
+#pragma unroll
+                for (int c = 0; c < PC; c++) {
+                    double u[3];
+                    u_of(c, u);
+                    for (int k = 0; k < 3; k++) uj[k] += u[k] * lj[3 + c];
+                }
+            }
+            const double E_b = ggx_sums_b(t, E, uj, n, v, w, mt.k, n_b, v_b, w_b, k_b);
+            if constexpr (VIS) vis_b[p * L + j] = (float)(E_b * E0);
+            const double r_b = -2.0 * E_b * E / r;
+            for (int k = 0; k < 3; k++) d_b[k] += r_b * w[k];
+            normalize_b(w, w_b, r, d_b);
+            for (int k = 0; k < 3; k++) x_b[k] -= d_b[k];
+        }
+    // m = mf (M / a), r = rf (R / a), k = r^4
+    const double r_b = k_b * (4.0 * ((mt.r * mt.r) * mt.r));
+    acc[4] += m_b * mt.M;
+    acc[5] += r_b * mt.R;
+    if (mr) {
+        mr_b[2 * p] = (float)(r_b * prm[5] / a);
+        mr_b[2 * p + 1] = (float)(m_b * prm[4] / a);
+        a_b -= (r_b * mt.r + m_b * mt.m) / a;
+    }
+    double dv_b[3] = {0, 0, 0}, N_b[3] = {0, 0, 0};
+    normalize_b(v, v_b, dn, dv_b);  // v = normalize(cam - x)
+    for (int j = 0; j < 3; j++) {
+        x_b[j] -= dv_b[j];
+        if (CENTER) acc[PHONG_SUMS + j] += dv_b[j];
+    }
+    a_b -= dot(x_b, x) / a;  // x = X / a
+    if (nn != 0.0) normalize_b(n, n_b, nn, N_b);
+    for (int j = 0; j < 3; j++) {
+        pb[io.off_normal + j] = (float)N_b[j];
+        pb[io.off_position + j] = (float)(x_b[j] / a);
+    }
+    pb[io.off_coverage] = (float)a_b;
+}
+
 // image[c] = A[c] (ambient + diff) + spec + (1 - a) bg[c], one thread per pixel; with an environment of S > 0
 // channels, A[c] ((ambient + diff) + sh_c(n)).  minBlocks 0 is no hint (the G-buffer instances are unchanged); with a
 // separate albedo the default budget spills 8 bytes at S = 1 across the fp64 division calls, so those instances take
@@ -916,18 +1321,25 @@ __device__ __forceinline__ float &albedo_b_at(float *pb, const DeodrPhongIO &io,
 // j's diffuse and specular terms are multiplied by its visibility vis [H,W,L] (DESIGN.md section 14); with SUN, the
 // directional light's by sun_vis [H,W] (DESIGN.md section 15).  With SPEC (SPLIT only), the specular map's
 // raster spec_map [H,W,2] = (K, E) gives every specular term, the point lights' included, aks = ks K and e(p) =
-// e E / a in place of a ks and e (DESIGN.md section 17)
-template <int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false, bool SPEC = false>
+// e E / a in place of a ks and e (DESIGN.md section 17).  With GGX (SPLIT only), the metallic-roughness form
+// (ggx_shade) replaces the Phong one, and spec_map is the metallic-roughness map's raster (R, M), or NULL for the
+// factors alone (DESIGN.md section 18)
+template <int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false, bool SPEC = false, bool GGX = false>
 __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(DeodrPhongIO io, const double *sh,
                                                                   const float *albedo, const double *lights, int L,
                                                                   const float *vis = nullptr,
                                                                   const float *sun_vis = nullptr,
                                                                   const float *spec_map = nullptr) {
     static_assert(SPLIT || !SPEC, "a specular map is read beside a separate albedo");
+    static_assert(!GGX || (SPLIT && !SPEC), "the metallic-roughness form reads a separate albedo and no specular map");
     const long long p = (long long)blockIdx.x * NT + threadIdx.x;
     if (p >= (long long)io.H * io.W) return;
     const int C = io.C;
     const float *px = io.channels + p * gbuffer_stride<SPLIT>(C);
+    if constexpr (GGX) {
+        ggx_shade<S, P, VIS, SUN>(io, px, p, sh, albedo, lights, L, vis, sun_vis, spec_map, io.image + p * C);
+        return;
+    }
     PhongTerms t;
     phong_terms<SPEC>(px, io, io.params, io.camera_center, t, SPEC ? spec_map + 2 * p : nullptr);
     if constexpr (SUN) {
@@ -1016,13 +1428,17 @@ __global__ void __launch_bounds__(NT, SPLIT || P > 0 ? 1 : 0) k_phong_shade(Deod
 // With SPEC (SPLIT only), aks = ks K and e(p) = e E / a from spec_map [H,W,2] = (K, E): q and e_b(p), the
 // gradients of aks and e(p) summed over the main term and the point lights, give spec_map_b [H,W,2] = (q ks,
 // e_b(p) e / a) (0 where a = 0), ks_b += q K, e_b += e_b(p) E / a and a_b -= e_b(p) e(p) / a (DESIGN.md section 17).
-template <bool CENTER, int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false, bool SPEC = false>
-__global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P == 0) || SPEC ? 1 : 0)
+// With GGX (SPLIT only), ggx_shade_b takes each pixel, spec_map is the metallic-roughness map's raster (R, M) or
+// NULL, spec_map_b its gradient, and params_b[4..5] are mf_b and rf_b (DESIGN.md section 18).
+template <bool CENTER, int S, bool SPLIT, int P = 0, bool VIS = false, bool SUN = false, bool SPEC = false,
+          bool GGX = false>
+__global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P == 0) || SPEC || GGX ? 1 : 0)
     k_phong_shade_b(DeodrPhongIO io, Scratch *s, const double *sh, const float *albedo, float *albedo_b,
                     const double *lights, int L, const float *vis = nullptr, float *vis_b = nullptr,
                     const float *sun_vis = nullptr, float *sun_vis_b = nullptr, const float *spec_map = nullptr,
                     float *spec_map_b = nullptr) {
     static_assert(SPLIT || !SPEC, "a specular map is read beside a separate albedo");
+    static_assert(!GGX || (SPLIT && !SPEC), "the metallic-roughness form reads a separate albedo and no specular map");
     constexpr int NC = S > P ? S : P;
     constexpr int K = PHONG_SUMS + (CENTER ? 3 : 0);
     __shared__ double tot[K];
@@ -1034,6 +1450,11 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
     const double ks = prm[4], e = prm[5];
     const long long pixels = (long long)io.H * io.W;
     for (long long p = (long long)blockIdx.x * NT + threadIdx.x; p < pixels; p += (long long)gridDim.x * NT) {
+        if constexpr (GGX) {
+            ggx_shade_b<CENTER, S, P, VIS, SUN>(io, p, sh, albedo, albedo_b, lights, L, vis, vis_b, sun_vis,
+                                                sun_vis_b, spec_map, spec_map_b, acc);
+            continue;
+        }
         const float *px = io.channels + p * gbuffer_stride<SPLIT>(C);
         const float *g = io.image_b + p * C;
         float *pb = io.channels_b + p * gbuffer_stride<SPLIT>(C);
@@ -1261,9 +1682,12 @@ __global__ void __launch_bounds__(NT, S == 2 || S == 4 || (SUN && S == 3 && P ==
 
 // sh_b[k, s] = sum over the pixels of g_s Y_k(n), g_c = image_b[c] A[c] (S = 1: summed over the channels, in the
 // order of lum_b above), n = N / |N| (0 when |N| = 0).  A pass of its own over the G-buffer and image_b: 9 S
-// accumulators beside k_phong_shade_b's would cost that kernel its occupancy (DESIGN.md section 11).
-template <int S, bool SPLIT>
-__global__ void __launch_bounds__(NT) k_phong_sh_b(DeodrPhongIO io, Scratch *s, double *sh_b, const float *albedo) {
+// accumulators beside k_phong_shade_b's would cost that kernel its occupancy (DESIGN.md section 11).  With GGX, the
+// environment lights the diffuse lobe only: g_c is scaled by 1 - m, m = mf (M / a) from the map raster mr [H,W,2]
+// (mf without one), and is 0 where a = 0.
+template <int S, bool SPLIT, bool GGX = false>
+__global__ void __launch_bounds__(NT) k_phong_sh_b(DeodrPhongIO io, Scratch *s, double *sh_b, const float *albedo,
+                                                   const float *mr = nullptr) {
     constexpr int K = 9 * S;
     __shared__ double tot[K];
     double acc[K];
@@ -1286,6 +1710,12 @@ __global__ void __launch_bounds__(NT) k_phong_sh_b(DeodrPhongIO io, Scratch *s, 
 #pragma unroll
             for (int c = 0; c < S; c++) g[c] = (double)albedo_at<SPLIT>(px, io, albedo, p, c) * (double)gp[c];
         }
+        if constexpr (GGX) {
+            const double a = px[io.off_coverage];
+            const double kd = a != 0.0 ? 1.0 - io.params[4] * (mr ? (double)mr[2 * p + 1] / a : 1.0) : 0.0;
+#pragma unroll
+            for (int c = 0; c < S; c++) g[c] *= kd;
+        }
 #pragma unroll
         for (int k = 0; k < 9; k++)
 #pragma unroll
@@ -1299,9 +1729,10 @@ __global__ void __launch_bounds__(NT) k_phong_sh_b(DeodrPhongIO io, Scratch *s, 
 // (the d_j share of k_phong_shade_b) and the intensity's, g_c A_c diff_j + g_c spec_j (P = 1: summed over the
 // channels); grid_sum_rows adds the CTAs in a fixed order.  The CTAs of one set of pixels are adjacent in the grid, so
 // the G-buffer is read from DRAM about once.  With VIS, light j's terms are scaled by vis [H,W,L].  With SPEC, the
-// terms use aks = ks K and e(p) = e E / a from spec_map [H,W,2]; the map's gradient is k_phong_shade_b's.
-template <int P, bool SPLIT, bool VIS = false, bool SPEC = false>
-__global__ void __launch_bounds__(NT) k_point_lights_pixel_b(DeodrPhongIO io, const float *albedo,
+// terms use aks = ks K and e(p) = e E / a from spec_map [H,W,2]; the map's gradient is k_phong_shade_b's.  With GGX,
+// the terms are the metallic-roughness form's (ggx_sums_b), with spec_map the map raster (R, M) or NULL.
+template <int P, bool SPLIT, bool VIS = false, bool SPEC = false, bool GGX = false>
+__global__ void __launch_bounds__(NT, GGX ? 1 : 0) k_point_lights_pixel_b(DeodrPhongIO io, const float *albedo,
                                                              const double *lights, double *lights_b, Scratch *s,
                                                              const float *vis = nullptr,
                                                              const float *spec_map = nullptr) {
@@ -1328,6 +1759,58 @@ __global__ void __launch_bounds__(NT) k_point_lights_pixel_b(DeodrPhongIO io, co
         }
         const double dn = sqrt(dot(v, v));
         for (int j = 0; j < 3; j++) v[j] /= dn;
+        if constexpr (GGX) {
+            // u[k][c]: the gradients of light j's three sums, per channel (P > 1) or summed (P = 1), as ggx_shade_b
+            GgxMaterial mt;
+            ggx_material(io.params, a, spec_map, p, mt);
+            const double kd = 1.0 - mt.m;
+            auto u_of = [&](int c, double u[3]) {
+                const double A = albedo[p * C + c], gc = g[c], F0 = 0.04 * kd + mt.m * (A / a);
+                u[0] = gc * (kd * A) * (1.0 - F0);
+                u[1] = gc * (a * F0);
+                u[2] = gc * a;
+            };
+            double d[3], w[3], w_b[3] = {0, 0, 0}, d_b[3] = {0, 0, 0}, n_b[3] = {0, 0, 0}, v_b[3] = {0, 0, 0}, k_b = 0;
+            double uj[3], tt[3];
+            for (int k = 0; k < 3; k++) d[k] = lj[k] - x[k];
+            const double r2 = dot(d, d), r = sqrt(r2);
+            if (!(r > 0)) continue;
+            for (int k = 0; k < 3; k++) w[k] = d[k] / r;
+            GgxTerm t;
+            ggx_term(n, v, w, mt.k, t);
+            const double vj = VIS ? (double)vis[p * gridDim.x + blockIdx.x] : 1.0;
+            const double E0 = (P == 1 ? lj[3] : 1.0) / r2, E = VIS ? E0 * vj : E0;
+            for (int k = 0; k < 3; k++) uj[k] = 0;
+            auto add_u = [&](int c) {
+                double u[3];
+                u_of(c, u);
+                for (int k = 0; k < 3; k++) uj[k] += u[k] * (P == 1 ? 1.0 : lj[3 + c]);
+            };
+            if (P > 1) {
+#pragma unroll
+                for (int c = 0; c < P; c++) add_u(c);
+            } else {
+                for (int c = 0; c < C; c++) add_u(c);
+            }
+            const double E_b = ggx_sums_b(t, E, uj, n, v, w, mt.k, n_b, v_b, w_b, k_b);
+            const double r_b = -2.0 * E_b * E / r;
+            for (int k = 0; k < 3; k++) d_b[k] += r_b * w[k];
+            normalize_b(w, w_b, r, d_b);
+            for (int k = 0; k < 3; k++) acc[k] += d_b[k];
+            // the intensity's: the sums at E = V / r^2
+            ggx_sums(t, VIS ? vj / r2 : 1.0 / r2, tt);
+            if (P > 1) {
+#pragma unroll
+                for (int c = 0; c < P; c++) {
+                    double u[3];
+                    u_of(c, u);
+                    acc[3 + c] += (u[0] * tt[0] + u[1] * tt[1]) + u[2] * tt[2];
+                }
+            } else {
+                acc[3] += (uj[0] * tt[0] + uj[1] * tt[1]) + uj[2] * tt[2];
+            }
+            continue;
+        }
         if (P > 1) {
 #pragma unroll
             for (int c = 0; c < P; c++) {
@@ -1447,20 +1930,21 @@ void launch_sh_lit_b(const double *normals, const double *vcol, int n, int C, co
                                                      sh_b, s);
 }
 
-template <int S, bool SPLIT = false, bool SUN = false, bool SPEC = false>
+template <int S, bool SPLIT = false, bool SUN = false, bool SPEC = false, bool GGX = false>
 void launch_phong_b(const DeodrPhongIO &io, const double *sh, double *sh_b, Scratch *s, cudaStream_t st,
                     const float *albedo = nullptr, float *albedo_b = nullptr, const float *sun_vis = nullptr,
                     float *sun_vis_b = nullptr, const float *spec_map = nullptr, float *spec_map_b = nullptr) {
     const long long pixels = (long long)io.H * io.W;
     const int g = reduce_grid(pixels);
     if (io.camera_center_b)
-        k_phong_shade_b<true, S, SPLIT, 0, false, SUN, SPEC><<<g, NT, 0, st>>>(
+        k_phong_shade_b<true, S, SPLIT, 0, false, SUN, SPEC, GGX><<<g, NT, 0, st>>>(
             io, s, sh, albedo, albedo_b, nullptr, 0, nullptr, nullptr, sun_vis, sun_vis_b, spec_map, spec_map_b);
     else
-        k_phong_shade_b<false, S, SPLIT, 0, false, SUN, SPEC><<<g, NT, 0, st>>>(
+        k_phong_shade_b<false, S, SPLIT, 0, false, SUN, SPEC, GGX><<<g, NT, 0, st>>>(
             io, s, sh, albedo, albedo_b, nullptr, 0, nullptr, nullptr, sun_vis, sun_vis_b, spec_map, spec_map_b);
     if constexpr (S > 0)
-        k_phong_sh_b<S, SPLIT><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo);
+        k_phong_sh_b<S, SPLIT, GGX><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo,
+                                                                                           GGX ? spec_map : nullptr);
 }
 
 // point lights of P channels for C colour channels: grey (P = 1), or one intensity per channel up to 4
@@ -1502,7 +1986,7 @@ dim3 light_grid(long long items, int L, int P) {
     return dim3(L, std::max(1, std::min(reduce_grid(items), MAX_K * MAX_CTAS / (L * (3 + P)))));
 }
 
-template <int S, int P, bool SPLIT, bool VIS = false, bool SUN = false, bool SPEC = false>
+template <int S, int P, bool SPLIT, bool VIS = false, bool SUN = false, bool SPEC = false, bool GGX = false>
 void launch_point_phong_b(const DeodrPhongIO &io, const float *albedo, float *albedo_b, const double *sh,
                           double *sh_b, const double *lights, int L, double *lights_b, Scratch *s, cudaStream_t st,
                           const float *vis = nullptr, float *vis_b = nullptr, const float *sun_vis = nullptr,
@@ -1510,17 +1994,18 @@ void launch_point_phong_b(const DeodrPhongIO &io, const float *albedo, float *al
     const long long pixels = (long long)io.H * io.W;
     const int g = reduce_grid(pixels);
     if (io.camera_center_b)
-        k_phong_shade_b<true, S, SPLIT, P, VIS, SUN, SPEC><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L,
-                                                                             vis, vis_b, sun_vis, sun_vis_b, spec_map,
-                                                                             spec_map_b);
+        k_phong_shade_b<true, S, SPLIT, P, VIS, SUN, SPEC, GGX><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights,
+                                                                                  L, vis, vis_b, sun_vis, sun_vis_b,
+                                                                                  spec_map, spec_map_b);
     else
-        k_phong_shade_b<false, S, SPLIT, P, VIS, SUN, SPEC><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights, L,
-                                                                              vis, vis_b, sun_vis, sun_vis_b, spec_map,
-                                                                              spec_map_b);
+        k_phong_shade_b<false, S, SPLIT, P, VIS, SUN, SPEC, GGX><<<g, NT, 0, st>>>(io, s, sh, albedo, albedo_b, lights,
+                                                                                   L, vis, vis_b, sun_vis, sun_vis_b,
+                                                                                   spec_map, spec_map_b);
     if constexpr (S > 0)
-        k_phong_sh_b<S, SPLIT><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo);
-    k_point_lights_pixel_b<P, SPLIT, VIS, SPEC><<<light_grid(pixels, L, P), NT, 0, st>>>(io, albedo, lights, lights_b,
-                                                                                         s, vis, spec_map);
+        k_phong_sh_b<S, SPLIT, GGX><<<std::min(g, MAX_K * MAX_CTAS / (9 * S)), NT, 0, st>>>(io, s, sh_b, albedo,
+                                                                                           GGX ? spec_map : nullptr);
+    k_point_lights_pixel_b<P, SPLIT, VIS, SPEC, GGX><<<light_grid(pixels, L, P), NT, 0, st>>>(
+        io, albedo, lights, lights_b, s, vis, spec_map);
 }
 
 }  // namespace
@@ -2123,6 +2608,81 @@ int deodr_b200_phong_shade_specular_map_b(const DeodrPhongIO *io, const float *a
                 launch_point_phong_b<S, P, true, VIS, SUN, true>(*io, albedo, albedo_b, sh, sh_b, lights, nb_lights,
                                                                  lights_b, s, st, vis, vis_b, sun_vis, sun_vis_b,
                                                                  spec, spec_b);
+            });
+        });
+    });
+    return check_launch();
+}
+
+int deodr_b200_pbr_shade(const DeodrPhongIO *io, const float *albedo, const float *mr, const double *sh,
+                         int sh_channels, const double *lights, int nb_lights, int light_channels, const float *vis,
+                         const float *sun_vis, void *stream) {
+    if (!phong_io_ok(io, true) || !io->image || !albedo || (!sh && sh_channels != 0) ||
+        (!lights && (nb_lights != 0 || vis)))
+        return bad("pbr_shade: bad argument (H, W >= 1, C in [1, 32760], off_albedo -1 and the other offsets tiling "
+                   "[0, 7), channels, params, camera_center, background, image and albedo non-NULL, sh NULL only "
+                   "with sh_channels 0, lights NULL only with nb_lights 0 and no vis)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) ||
+        (lights && (!light_channels_ok(light_channels, io->C) || nb_lights < 1 || nb_lights > MAX_LIGHTS)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "pbr_shade: nb_lights must be 1 to 8, and sh_channels and "
+                                                  "light_channels 1, or C from 1 to 4");
+    const int g = grid_of((long long)io->H * io->W);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S_ = sh ? sh_channels : 0;
+    if (!lights) {
+        with_sh_channels(S_, [&](auto S) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                k_phong_shade<S, true, 0, false, SUN, false, true><<<g, NT, 0, st>>>(*io, sh, albedo, nullptr, 0,
+                                                                                     nullptr, sun_vis, mr);
+            });
+        });
+        return check_launch();
+    }
+    with_point_channels(S_, light_channels, [&](auto S, auto P) {
+        with_flag(vis != nullptr, [&](auto VIS) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                k_phong_shade<S, true, P, VIS, SUN, false, true><<<g, NT, 0, st>>>(*io, sh, albedo, lights,
+                                                                                   nb_lights, vis, sun_vis, mr);
+            });
+        });
+    });
+    return check_launch();
+}
+
+int deodr_b200_pbr_shade_b(const DeodrPhongIO *io, const float *albedo, const float *mr, const double *sh,
+                           int sh_channels, const double *lights, int nb_lights, int light_channels, const float *vis,
+                           const float *sun_vis, float *albedo_b, float *mr_b, double *sh_b, double *lights_b,
+                           float *vis_b, float *sun_vis_b, double *scratch, void *stream) {
+    if (!phong_io_ok(io, true) || !io->image_b || !io->channels_b || !io->params_b || !albedo || !albedo_b ||
+        (!mr != !mr_b) || (!sh && sh_channels != 0) || (sh && !sh_b) || (!lights && (nb_lights != 0 || vis)) ||
+        (lights && !lights_b) || (vis && !vis_b) || (sun_vis && !sun_vis_b) || !scratch)
+        return bad("pbr_shade_b: bad argument (H, W >= 1, C in [1, 32760], off_albedo -1 and the other offsets "
+                   "tiling [0, 7), channels, params, camera_center, background, image_b, channels_b, params_b, "
+                   "albedo, albedo_b and scratch non-NULL, mr_b non-NULL exactly with mr, sh NULL only with "
+                   "sh_channels 0, sh_b non-NULL with sh, lights NULL only with nb_lights 0 and no vis, lights_b "
+                   "non-NULL with lights, vis_b with vis, sun_vis_b with sun_vis)");
+    if ((sh && !sh_channels_ok(sh_channels, io->C)) ||
+        (lights && (!light_channels_ok(light_channels, io->C) || nb_lights < 1 || nb_lights > MAX_LIGHTS)))
+        return set_error(DEODR_B200_EUNSUPPORTED, "pbr_shade_b: nb_lights must be 1 to 8, and sh_channels and "
+                                                  "light_channels 1, or C from 1 to 4");
+    Scratch *s = reinterpret_cast<Scratch *>(scratch);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S_ = sh ? sh_channels : 0;
+    if (!lights) {
+        with_sh_channels(S_, [&](auto S) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                launch_phong_b<S, true, SUN, false, true>(*io, sh, sh_b, s, st, albedo, albedo_b, sun_vis, sun_vis_b,
+                                                          mr, mr_b);
+            });
+        });
+        return check_launch();
+    }
+    with_point_channels(S_, light_channels, [&](auto S, auto P) {
+        with_flag(vis != nullptr, [&](auto VIS) {
+            with_flag(sun_vis != nullptr, [&](auto SUN) {
+                launch_point_phong_b<S, P, true, VIS, SUN, false, true>(*io, albedo, albedo_b, sh, sh_b, lights,
+                                                                        nb_lights, lights_b, s, st, vis, vis_b,
+                                                                        sun_vis, sun_vis_b, mr, mr_b);
             });
         });
     });

@@ -437,7 +437,7 @@ def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: tor
                 albedo: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None,
                 visibility: Optional[torch.Tensor] = None,
                 sun_visibility: Optional[torch.Tensor] = None,
-                specular: Optional[torch.Tensor] = None) -> torch.Tensor:
+                specular: Optional[torch.Tensor] = None, brdf: str = "phong") -> torch.Tensor:
     """The per-pixel shading of a G-buffer (deodr_b200_phong_shade, or deodr_b200_sh_phong_shade with ``sh``; model in
     include/deodr_b200.h): ``channels``
     [H,W,C+7] f32 laid out (albedo C, normal 3, position 3, coverage 1), ``params`` [6] fp64 on the device = (light
@@ -451,12 +451,31 @@ def phong_shade(channels: torch.Tensor, params: torch.Tensor, camera_center: tor
     [H,W] f32 (:func:`sun_visibility`), which multiplies its diffuse and specular terms, with or without an
     environment, point lights and their ``visibility`` (deodr_b200_phong_shade_sun_shadowed).  ``specular``: with an
     albedo, the specular map's raster [H,W,2] = (K, E) (the model in include/deodr_b200.h), which gives every specular
-    term aks = ks K and e(p) = e E / a, with any of the inputs above (deodr_b200_phong_shade_specular_map)."""
+    term aks = ks K and e(p) = e E / a, with any of the inputs above (deodr_b200_phong_shade_specular_map).
+    ``brdf="ggx"`` is the metallic-roughness form instead (deodr_b200_pbr_shade; the model in include/deodr_b200.h):
+    it needs an albedo, ``params`` [6] = (light, ambient, metallic mf, roughness rf), and ``specular`` is then the
+    metallic-roughness map's raster [H,W,2] = (R, M) or None (the factors alone)."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     H, W = keep[0].shape[:2]
     image = torch.empty((H, W, io.C), dtype=torch.float32, device=keep[0].device)
     io.image = image.data_ptr()
-    if specular is not None:
+    if brdf not in ("phong", "ggx"):
+        raise ValueError(f"brdf must be 'phong' or 'ggx'; got {brdf!r}")
+    if brdf == "ggx":
+        if albedo is None:
+            raise ValueError("the metallic-roughness form reads a separate albedo (a textured view's)")
+        mr = _check_specular(specular, albedo, H, W, image.device) if specular is not None else None
+        sun = _check_sun_visibility(sun_visibility, H, W, image.device) if sun_visibility is not None else None
+        lights, L, P = _check_point_lights(point_lights, image.device) if point_lights is not None else (None, 0, 0)
+        vis = _check_visibility(visibility, H, W, L, image.device) if visibility is not None else None
+        if vis is not None and lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        sh, S = _check_sh(sh, image.device) if sh is not None else (None, 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        _cabi.check(_cabi.load().deodr_b200_pbr_shade(
+            C.byref(io), keep[4].data_ptr(), ptr(mr), ptr(sh), S, ptr(lights), L, P, ptr(vis), ptr(sun),
+            _stream(image.device)))
+    elif specular is not None:
         spec = _check_specular(specular, albedo, H, W, image.device)
         sun = _check_sun_visibility(sun_visibility, H, W, image.device) if sun_visibility is not None else None
         lights, L, P = _check_point_lights(point_lights, image.device) if point_lights is not None else (None, 0, 0)
@@ -515,7 +534,7 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
                          point_lights: Optional[torch.Tensor] = None,
                          visibility: Optional[torch.Tensor] = None,
                          sun_visibility: Optional[torch.Tensor] = None,
-                         specular: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, ...]:
+                         specular: Optional[torch.Tensor] = None, brdf: str = "phong") -> Tuple[torch.Tensor, ...]:
     """-> (channels_b [H,W,C+7] f32, params_b [6] fp64), the adjoint of :func:`phong_shade` from ``image_b`` [H,W,C]
     (deodr_b200_phong_shade_b, or deodr_b200_sh_phong_shade_b with ``sh``).  channels_b includes the coverage channel's gradient; ``params_b`` is summed over the
     pixels in a fixed order (bit-reproducible).  ``scratch``: a buffer of ``mesh_fitter.new_scratch``.  With
@@ -526,7 +545,9 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     in a fixed order (deodr_b200_point_phong_shade_b); with ``visibility`` too it then ends with vis_b [H,W,L] f32
     (deodr_b200_point_phong_shade_shadowed_b).  With ``sun_visibility`` the result ends with sun_vis_b [H,W] f32
     (deodr_b200_phong_shade_sun_shadowed_b).  With ``specular`` (the map raster of :func:`phong_shade`) it ends with
-    spec_b [H,W,2] f32 (deodr_b200_phong_shade_specular_map_b)."""
+    spec_b [H,W,2] f32 (deodr_b200_phong_shade_specular_map_b).  With ``brdf="ggx"`` it is the adjoint of the
+    metallic-roughness form (deodr_b200_pbr_shade_b): params_b[4:6] are the metallic and roughness factors' gradients,
+    and with a map raster ``specular`` the result ends with its gradient mr_b [H,W,2] f32."""
     io, keep = _phong_io(channels, params, camera_center, background, albedo)
     dev = keep[0].device
     S = _check_sh(sh, dev)[1] if sh is not None else 0
@@ -546,7 +567,26 @@ def phong_shade_backward(channels: torch.Tensor, params: torch.Tensor, camera_ce
     if albedo is not None:
         albedo_b = torch.empty((H, W, io.C), dtype=torch.float32, device=dev)
     lights_b = vis_b = sun_b = spec_b = None
-    if specular is not None:
+    if brdf not in ("phong", "ggx"):
+        raise ValueError(f"brdf must be 'phong' or 'ggx'; got {brdf!r}")
+    if brdf == "ggx":
+        if albedo is None:
+            raise ValueError("the metallic-roughness form reads a separate albedo (a textured view's)")
+        mr = _check_specular(specular, albedo, H, W, dev) if specular is not None else None
+        sun = _check_sun_visibility(sun_visibility, H, W, dev) if sun_visibility is not None else None
+        lights, L, P = _check_point_lights(point_lights, dev) if point_lights is not None else (None, 0, 0)
+        vis = _check_visibility(visibility, H, W, L, dev) if visibility is not None else None
+        if vis is not None and lights is None:
+            raise ValueError("visibility multiplies the point lights' terms: it needs point_lights")
+        lights_b = torch.empty_like(lights) if lights is not None else None
+        vis_b = torch.empty((H, W, L), dtype=torch.float32, device=dev) if vis is not None else None
+        sun_b = torch.empty((H, W), dtype=torch.float32, device=dev) if sun is not None else None
+        spec_b = torch.empty((H, W, 2), dtype=torch.float32, device=dev) if mr is not None else None
+        _cabi.check(_cabi.load().deodr_b200_pbr_shade_b(
+            C.byref(io), keep[4].data_ptr(), ptr(mr), ptr(sh), S, ptr(lights), L, P, ptr(vis), ptr(sun),
+            albedo_b.data_ptr(), ptr(spec_b), ptr(sh_b), ptr(lights_b), ptr(vis_b), ptr(sun_b),
+            scratch.data_ptr(), _stream(dev)))
+    elif specular is not None:
         spec = _check_specular(specular, albedo, H, W, dev)
         sun = _check_sun_visibility(sun_visibility, H, W, dev) if sun_visibility is not None else None
         lights, L, P = _check_point_lights(point_lights, dev) if point_lights is not None else (None, 0, 0)
@@ -1274,9 +1314,9 @@ def check_shadow_arguments(shading: str, point_lights, size: int, bias, softness
     size = int(size)
     if size == 0:
         return 0
-    if shading not in ("phong", "phong_textured"):
-        raise ValueError("shadows need per-pixel shading (shading='phong' or 'phong_textured'): a shadow edge crosses "
-                         "triangles, and per-vertex visibility would smear it over each one")
+    if shading not in ("phong", "phong_textured", "pbr_textured"):
+        raise ValueError("shadows need per-pixel shading (shading='phong', 'phong_textured' or 'pbr_textured'): a "
+                         "shadow edge crosses triangles, and per-vertex visibility would smear it over each one")
     if point_lights is None:
         raise ValueError("shadows are cast from point lights: this view has none")
     if not SHADOW_MAP_SIZES[0] <= size <= SHADOW_MAP_SIZES[1]:
@@ -1293,9 +1333,9 @@ def check_sun_shadow_arguments(shading: str, light_directional, size: int, bias,
     size = int(size)
     if size == 0:
         return 0
-    if shading not in ("phong", "phong_textured"):
-        raise ValueError("light shadows need per-pixel shading (shading='phong' or 'phong_textured'): a shadow edge "
-                         "crosses triangles, and per-vertex visibility would smear it over each one")
+    if shading not in ("phong", "phong_textured", "pbr_textured"):
+        raise ValueError("light shadows need per-pixel shading (shading='phong', 'phong_textured' or 'pbr_textured'): "
+                         "a shadow edge crosses triangles, and per-vertex visibility would smear it over each one")
     if light_directional is None:
         raise ValueError("light shadows are cast from the directional light: this view has none")
     if not SHADOW_MAP_SIZES[0] <= size <= SHADOW_MAP_SIZES[1]:
@@ -1482,6 +1522,16 @@ class DeviceMeshView:
     ``specular_map_b`` [Ht,Wt,2] f32 and the map raster's share of ``uv_b`` and of the vertices' gradient.
     ``render(..., specular_map=)`` copies a new map in.  Every other shading refuses a specular map.
 
+    ``shading="pbr_textured"`` shades a textured view per pixel with a metallic-roughness material (a GGX highlight
+    coloured by the metal, the model in include/deodr_b200.h): the factors ``metallic`` (default 0) and ``roughness``
+    (default 0.5), and an optional ``metallic_roughness_map`` [Ht,Wt,2] = (roughness_t, metallic_t) per texel that
+    multiplies them (glTF's factor x texture; its G and B channels).  Every other layer is the textured Phong view's:
+    the map's raster takes the specular map's place, and normal maps, environments, point lights and both kinds of
+    shadows compose with it.  :meth:`backward` returns ``material_b`` [2] = (metallic_b, roughness_b) in place of
+    ``specular_b``, and ``metallic_roughness_map_b`` [Ht,Wt,2] f32 with a map.  ``render(..., metallic_roughness_map=)``
+    copies a new map in.  The view refuses ``specular``, ``shininess`` and ``specular_map``; every other shading
+    refuses ``metallic``, ``roughness`` and a metallic-roughness map.
+
     ``camera`` is a :class:`CameraParams`, or a camera vector [26] fp64 tensor on the view's device (extrinsic,
     intrinsic, distortion; ``has_distortion`` says whether its distortion is applied).  A tensor is read at every
     render, so a fit can update it in place between steps without a host read.  ``backward(..., camera_grad=True)``
@@ -1527,19 +1577,31 @@ class DeviceMeshView:
                  light_directional=None, ambient: float = 1.0, background_color=(0.0, 0.0, 0.0), sigma: float = 1.0,
                  clockwise: bool = False, device="cuda", slot: int = 0, uv=None, faces_uv=None, texture=None,
                  backface_culling: bool = True, perspective_correct: bool = False, shading: str = "gouraud",
-                 specular: float = 0.0, shininess: float = 16.0, has_distortion: bool = True,
+                 specular: Optional[float] = None, shininess: Optional[float] = None, has_distortion: bool = True,
                  sh: Optional[torch.Tensor] = None, point_lights: Optional[torch.Tensor] = None,
                  shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
                  shadow_softness: Optional[float] = None, light_shadow_map_size: int = 0,
                  light_shadow_bias: Optional[float] = None, light_shadow_softness: Optional[float] = None,
-                 light_shadow_bounds=None, normal_map=None, specular_map=None):
+                 light_shadow_bounds=None, normal_map=None, specular_map=None, metallic: Optional[float] = None,
+                 roughness: Optional[float] = None, metallic_roughness_map=None):
         from .renderer import DeviceScene, default_renderer
         from .scenes import SceneArrays
 
         nb_colors = len(background_color)
         textured = uv is not None or faces_uv is not None or texture is not None
-        if shading not in ("gouraud", "phong", "phong_textured"):
-            raise ValueError(f"shading must be 'gouraud', 'phong' or 'phong_textured'; got {shading!r}")
+        if shading not in ("gouraud", "phong", "phong_textured", "pbr_textured"):
+            raise ValueError(f"shading must be 'gouraud', 'phong', 'phong_textured' or 'pbr_textured'; got {shading!r}")
+        self.pbr = shading == "pbr_textured"
+        if self.pbr:
+            if not textured:
+                raise ValueError("shading='pbr_textured' needs a textured view (uv, faces_uv and texture)")
+            if specular is not None or shininess is not None or specular_map is not None:
+                raise ValueError("a 'pbr_textured' view takes metallic, roughness and metallic_roughness_map, not the "
+                                 "Phong form's specular, shininess or specular_map")
+        elif metallic is not None or roughness is not None or metallic_roughness_map is not None:
+            raise ValueError("metallic, roughness and metallic_roughness_map need shading='pbr_textured'")
+        # the textured per-pixel forms share every layer but the shading kernel
+        per_pixel_textured = shading in ("phong_textured", "pbr_textured")
         if shading == "phong" and textured:
             raise ValueError("phong shading of a textured mesh is shading='phong_textured' (its albedo is a raster of "
                              "its own)")
@@ -1548,12 +1610,16 @@ class DeviceMeshView:
                              "view takes shading='phong'")
         if shading != "gouraud" and perspective_correct:
             raise ValueError("phong shading interpolates linearly in screen space; perspective_correct is refused")
-        self.shading, self.specular, self.shininess = shading, float(specular), float(shininess)
+        self.shading = shading
+        self.specular = 0.0 if specular is None else float(specular)
+        self.shininess = 16.0 if shininess is None else float(shininess)
+        self.metallic = 0.0 if metallic is None else float(metallic)
+        self.roughness = 0.5 if roughness is None else float(roughness)
         if sh is not None:
             S = _check_sh(sh, torch.device(device))[1]
             if S != 1 and (S != nb_colors or S > 4):
                 raise ValueError(f"sh must be [9], or [9,C] with C = {nb_colors} from 1 to 4; got {tuple(sh.shape)}")
-            if textured and S != 1 and shading != "phong_textured":
+            if textured and S != 1 and not per_pixel_textured:
                 raise ValueError("a textured view takes a grey environment [9] only: its shade has one channel (or "
                                  "shading='phong_textured')")
         self.sh = sh
@@ -1562,7 +1628,7 @@ class DeviceMeshView:
             if S != 1 and (S != nb_colors or S > 4):
                 raise ValueError(f"point lights must be [L, 4], or [L, 3 + C] with C = {nb_colors} from 1 to 4; got "
                                  f"{tuple(point_lights.shape)}")
-            if textured and S != 1 and shading != "phong_textured":
+            if textured and S != 1 and not per_pixel_textured:
                 raise ValueError("a textured view takes grey point lights [L, 4] only: its shade has one channel (or "
                                  "shading='phong_textured')")
         self.point_lights = point_lights
@@ -1590,9 +1656,9 @@ class DeviceMeshView:
             if uv.ndim != 2 or uv.shape[1] != 2 or faces_uv.shape != np.shape(faces):
                 raise ValueError("uv must be [Nuv,2] and faces_uv [T,3] like faces")
         if normal_map is not None:
-            if shading != "phong_textured":
+            if not per_pixel_textured:
                 raise ValueError("a normal map perturbs the per-pixel normal of a textured view: it needs "
-                                 "shading='phong_textured'")
+                                 "shading='phong_textured' or 'pbr_textured'")
             normal_map = np.asarray(normal_map.detach().cpu() if isinstance(normal_map, torch.Tensor) else normal_map,
                                     dtype=np.float64)
             if normal_map.shape != texture.shape[:2] + (3,):
@@ -1609,6 +1675,17 @@ class DeviceMeshView:
                 raise ValueError(f"specular_map must be [Ht,Wt,2] with the texture's Ht and Wt = {texture.shape[:2]}; "
                                  f"got shape {specular_map.shape}")
         self.specular_mapped = specular_map is not None
+        if metallic_roughness_map is not None:
+            metallic_roughness_map = np.asarray(
+                metallic_roughness_map.detach().cpu() if isinstance(metallic_roughness_map, torch.Tensor)
+                else metallic_roughness_map, dtype=np.float64)
+            if metallic_roughness_map.shape != texture.shape[:2] + (2,):
+                raise ValueError(f"metallic_roughness_map must be [Ht,Wt,2] with the texture's Ht and Wt = "
+                                 f"{texture.shape[:2]}; got shape {metallic_roughness_map.shape}")
+        self.metallic_roughness_mapped = metallic_roughness_map is not None
+        # a specular map or a metallic-roughness map: one 2-channel raster beside the albedo (a view has at most one)
+        material_map = specular_map if specular_map is not None else metallic_roughness_map
+        self._material_mapped = material_map is not None
         self.device = torch.device(device)
         self.topology = MeshTopology(faces, nb_vertices, clockwise=clockwise, device=self.device)
         self.camera, self.sigma = camera, float(sigma)
@@ -1624,7 +1701,7 @@ class DeviceMeshView:
         T, V = faces_u32.shape[0], int(nb_vertices)
         flags = np.ones(T, bool) if textured else np.zeros(T, bool)
         # a textured Phong view's scene is its albedo raster: a shade of 1, set here once, over a zero background
-        albedo_raster = shading == "phong_textured"
+        albedo_raster = per_pixel_textured
         background = np.asarray(background_color, dtype=np.float64)
         arrays = SceneArrays(
             faces=faces_u32, faces_uv=faces_uv if textured else np.zeros((T, 3), np.uint32), ij=np.zeros((V, 2)),
@@ -1681,12 +1758,12 @@ class DeviceMeshView:
                 background_color=np.zeros(3), clockwise=clockwise, backface_culling=bool(backface_culling),
                 strict_edge=True, perspective_correct=False, integer_pixel_centers=True), self.device)
             self._tangents = VertexTangents(self.topology, faces_uv, uv.shape[0])
-        if self.specular_mapped:
-            # the specular map's raster: the albedo raster's arrays with the map as a 2-channel texture
+        if self._material_mapped:
+            # the material map's raster: the albedo raster's arrays with the map as a 2-channel texture
             self._spec_scene = DeviceScene(SceneArrays(
                 faces=faces_u32, faces_uv=faces_uv, ij=np.zeros((V, 2)), depths=np.ones(V), textured=flags, uv=uv,
                 shade=np.ones(V), colors=np.zeros((V, 2)), shaded=flags, edgeflags=np.zeros((T, 3), bool),
-                height=height, width=width, nb_colors=2, texture=specular_map, background_image=None,
+                height=height, width=width, nb_colors=2, texture=material_map, background_image=None,
                 background_color=np.zeros(2), clockwise=clockwise, backface_culling=bool(backface_culling),
                 strict_edge=True, perspective_correct=False, integer_pixel_centers=True), self.device)
         self._maps = []  # the shadow maps rendered beside the view's raster(s): the cube maps, then the sun map
@@ -1780,7 +1857,7 @@ class DeviceMeshView:
                                      self.light_shadow_softness, albedo=albedo)
         return phong_shade(gbuffer, params, center, background, sh=self.sh, albedo=albedo,
                            point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis,
-                           specular=spec), vis, sun_vis
+                           specular=spec, brdf="ggx" if self.pbr else "phong"), vis, sun_vis
 
     def _shade_backward(self, gbuffer, params, center, background, image_b, camera_grad, albedo, vis, sun_vis,
                         spec=None):
@@ -1790,7 +1867,7 @@ class DeviceMeshView:
         shaded = phong_shade_backward(gbuffer, params, center, background, image_b, self._phong_scratch,
                                       center_grad=camera_grad, sh=self.sh, albedo=albedo,
                                       point_lights=self.point_lights, visibility=vis, sun_visibility=sun_vis,
-                                      specular=spec)
+                                      specular=spec, brdf="ggx" if self.pbr else "phong")
         spec_b = None
         if spec is not None:
             shaded, spec_b = shaded[:-1], shaded[-1]
@@ -1812,11 +1889,13 @@ class DeviceMeshView:
         return shaded, maps_b, spec_b
 
     def _phong_params(self) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(params [6], camera_center [3]) fp64 on the device, uploaded again only when the light, the specular
-        parameters or the camera have changed since the last render (so that a render normally copies nothing)."""
+        """(params [6], camera_center [3]) fp64 on the device, uploaded again only when the light, the specular (or
+        metallic-roughness) parameters or the camera have changed since the last render (so that a render normally
+        copies nothing)."""
         l = (0.0, 0.0, 0.0) if self.light_directional is None else \
             tuple(np.asarray(self.light_directional, dtype=np.float64).reshape(3).tolist())
-        params = l + (float(self.ambient), float(self.specular), float(self.shininess))
+        material = (self.metallic, self.roughness) if self.pbr else (self.specular, self.shininess)
+        params = l + (float(self.ambient), float(material[0]), float(material[1]))
         if isinstance(self.camera, torch.Tensor):
             if self._phong_key != params:
                 self._phong_key = params
@@ -1884,12 +1963,13 @@ class DeviceMeshView:
 
     def render(self, vertices: torch.Tensor, vertex_colors: Optional[torch.Tensor] = None,
                texture: Optional[torch.Tensor] = None, normal_map: Optional[torch.Tensor] = None,
-               specular_map: Optional[torch.Tensor] = None) -> torch.Tensor:
+               specular_map: Optional[torch.Tensor] = None,
+               metallic_roughness_map: Optional[torch.Tensor] = None) -> torch.Tensor:
         """The image [H,W,C] f32 of the mesh at ``vertices`` [V,3]: Gouraud-lit ``vertex_colors`` [V,C] for an untextured
         view; for a textured one the texture shaded by the vertex luminosity, with ``texture`` [Ht,Wt,C] (if given)
         copied into the view's texture first, so that a fit can vary it.  ``normal_map`` [Ht,Wt,3], in a view made with
-        one, is copied into the view's normal map in the same way, and ``specular_map`` [Ht,Wt,2] into its specular
-        map."""
+        one, is copied into the view's normal map in the same way, ``specular_map`` [Ht,Wt,2] into its specular
+        map and ``metallic_roughness_map`` [Ht,Wt,2] into its metallic-roughness map."""
         if normal_map is not None:
             if not self.normal_mapped:
                 raise ValueError("this view has no normal map (DeviceMeshView(..., normal_map=) makes one)")
@@ -1904,10 +1984,18 @@ class DeviceMeshView:
                 raise ValueError(f"specular_map has shape {tuple(specular_map.shape)}, expected "
                                  f"{tuple(self._spec_scene.t['texture'].shape)}")
             self._spec_scene.t["texture"].copy_(specular_map)
+        if metallic_roughness_map is not None:
+            if not self.metallic_roughness_mapped:
+                raise ValueError("this view has no metallic-roughness map (DeviceMeshView(..., "
+                                 "metallic_roughness_map=) makes one)")
+            if tuple(metallic_roughness_map.shape) != tuple(self._spec_scene.t["texture"].shape):
+                raise ValueError(f"metallic_roughness_map has shape {tuple(metallic_roughness_map.shape)}, expected "
+                                 f"{tuple(self._spec_scene.t['texture'].shape)}")
+            self._spec_scene.t["texture"].copy_(metallic_roughness_map)
         if self.textured:
             if vertex_colors is not None:
                 raise ValueError("a textured view takes no vertex_colors (its colour is the shaded texture)")
-            if self.shading == "phong_textured":
+            if self.shading in ("phong_textured", "pbr_textured"):
                 return self._render_phong_textured(vertices, texture)
             return self._render_textured(vertices, texture)
         if vertex_colors is None:
@@ -2018,8 +2106,8 @@ class DeviceMeshView:
             m["depths"].copy_(depths)
             m["edgeflags"].copy_(a["edgeflags"])
             scenes.append(self._map_scene)
-        if self.specular_mapped:
-            # the specular map's raster, last, which shares the geometry too
+        if self._material_mapped:
+            # the material map's raster (specular or metallic-roughness), last, which shares the geometry too
             s = self._spec_scene.t
             s["ij"].copy_(ij)
             s["depths"].copy_(depths)
@@ -2028,7 +2116,7 @@ class DeviceMeshView:
         params, center = self._phong_params()
         fwds = self._render_with_maps(scenes, vertices, params)
         gbuffer = normal_map(fwds[1]["image"], fwds[2]["image"]) if self.normal_mapped else fwds[1]["image"]
-        spec = fwds[-1]["image"] if self.specular_mapped else None
+        spec = fwds[-1]["image"] if self._material_mapped else None
         image, vis, sun_vis = self._shade(gbuffer, params, center, self._phong_background, albedo=fwds[0]["image"],
                                           spec=spec)
         self._gbuffer = gbuffer
@@ -2043,10 +2131,10 @@ class DeviceMeshView:
         # with a normal map, the perturbation's adjoint first takes the 7-channel channels_b to the 13-channel
         # G-buffer's and the map raster's image gradients; the three rasters' adjoint is one call, the tangent slices
         # of colors_b go through the tangent frame's adjoint into vertices_b and uv_b, and the ij_b and uv_b summed.
-        # A specular map's raster, last, takes the shading's spec_b in the same adjoint call; its ij_b and uv_b are
-        # summed in too
+        # A material map's raster (specular or metallic-roughness), last, takes the shading's spec_b in the same
+        # adjoint call; its ij_b and uv_b are summed in too
         vertices, _, _, fwds, params, center, vis, sun_vis = self._saved
-        spec = fwds[-1]["image"] if self.specular_mapped else None
+        spec = fwds[-1]["image"] if self._material_mapped else None
         shaded, maps_b, spec_b = self._shade_backward(self._gbuffer, params, center, self._phong_background, image_b,
                                                       camera_grad, fwds[0]["image"], vis, sun_vis, spec)
         lights_b = None
@@ -2058,7 +2146,7 @@ class DeviceMeshView:
             image_bs[1], map_image_b = normal_map_backward(fwds[1]["image"], fwds[2]["image"], channels_b)
             scenes.append(self._map_scene)
             image_bs.append(map_image_b)
-        if self.specular_mapped:
+        if self._material_mapped:
             scenes.append(self._spec_scene)
             image_bs.append(spec_b)
         grads = self._render_b_with_maps(scenes, fwds, image_bs, maps_b)
@@ -2073,17 +2161,17 @@ class DeviceMeshView:
         ij_b = ga["ij_b"] + gg["ij_b"]
         if self.normal_mapped:
             ij_b = ij_b + grads[2]["ij_b"]
-        if self.specular_mapped:
+        if self._material_mapped:
             ij_b = ij_b + grads[-1]["ij_b"]
             uv_b = uv_b + grads[-1]["uv_b"]
         self._maps_backward(vertices, params, vertices_b, params_b, lights_b)
         _, camera_b = self._project_backward(vertices, ij_b, None, vertices_b, reference_transpose, camera_grad)
         out = {"vertices_b": vertices_b, "texture_b": ga["texture_b"], "uv_b": uv_b, "light_b": params_b[:4],
-               "specular_b": params_b[4:]}
+               "material_b" if self.pbr else "specular_b": params_b[4:]}
         if self.normal_mapped:
             out["normal_map_b"] = grads[2]["texture_b"]
-        if self.specular_mapped:
-            out["specular_map_b"] = grads[-1]["texture_b"]
+        if self._material_mapped:
+            out["metallic_roughness_map_b" if self.pbr else "specular_map_b"] = grads[-1]["texture_b"]
         if camera_grad:
             out.update(self._camera_result(camera_b, shaded[2]))
         if self.sh is not None:
@@ -2130,7 +2218,7 @@ class DeviceMeshView:
             raise ValueError("perspective_correct has no adjoint (as in the reference, Scene3D.render_backward)")
         if self.shading == "phong":
             return self._backward_phong(image_b, reference_transpose, camera_grad)
-        if self.shading == "phong_textured":
+        if self.shading in ("phong_textured", "pbr_textured"):
             return self._backward_phong_textured(image_b, reference_transpose, camera_grad)
         vertices, vertex_colors, normals, fwd = self._saved
         grads = self.renderer.render_b(self.scene, self.sigma, fwd, image_b)

@@ -30,14 +30,16 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
                            -> image [H,W,C] fp32, the per-pixel shading of a G-buffer; a centre tensor and sh receive
                            their gradients.  With a separate albedo the G-buffer is [H,W,7] and the albedo gets one;
                            point_lights [L, 3 + S] | None get theirs; the specular map's raster [H,W,2] | None (with
-                           the albedo) gives the per-pixel ks and e, and receives its gradient
+                           the albedo) gives the per-pixel ks and e, and receives its gradient.  brdf="ggx" is the
+                           metallic-roughness form: specular and shininess are the metallic and roughness factors,
+                           and the 2-channel raster is the metallic-roughness map's
     RenderMeshPhongTexturedFunc  (ij, uv, texture, channels [V,7], depths, edgeflags, albedo scene, G-buffer scene,
                            sigma) -> (albedo [H,W,C], G-buffer [H,W,7]): the two rasters of a textured Phong render
                            in one forward call and one adjoint call; gradients to ij, uv, texture and channels.  With
                            a normal map [Ht,Wt,3] and its scene, channels are [V,13] and a third raster, the map's
                            [H,W,3], is rendered in the same calls; the map receives its gradient.  With a specular map
-                           [Ht,Wt,2] and its scene, one more raster, the map's [H,W,2], is rendered last in the same
-                           calls; the map receives its gradient
+                           [Ht,Wt,2] (or a metallic-roughness map) and its scene, one more raster, the map's [H,W,2],
+                           is rendered last in the same calls; the map receives its gradient
     RenderShadowedPhongFunc  (ij, uv | None, texture | None, channels, depths, edgeflags, vertices, point_lights,
                            albedo scene | None, G-buffer scene, ShadowCubes, sigma) -> ([albedo,] G-buffer, cube maps
                            [6L,M,M]): a Phong render's raster(s) and the lights' cube shadow maps in one forward call
@@ -485,14 +487,17 @@ class PhongShadeFunc(torch.autograd.Function):
     parameter and centre gradients are summed over the pixels in a fixed order.  With ``albedo`` [H,W,C] (a textured
     mesh's albedo raster) the channels are [H,W,7] = (normal, position, coverage) and the albedo gets its gradient.
     ``specular_raster`` [H,W,2] (with the albedo) is the specular map's raster (K, E), which gives every specular term
-    aks = ks K and e(p) = e E / a (the model in include/deodr_b200.h), and gets its gradient."""
+    aks = ks K and e(p) = e E / a (the model in include/deodr_b200.h), and gets its gradient.  ``brdf="ggx"`` (with the
+    albedo) is the metallic-roughness form instead: ``specular`` and ``shininess`` are then the metallic and roughness
+    factors, and ``specular_raster`` the metallic-roughness map's raster (R, M) or None."""
 
     @staticmethod
     def forward(ctx: Any, channels: torch.Tensor, light_directional: Optional[torch.Tensor],  # type: ignore
                 light_ambient, specular, shininess, camera: CameraParams, background,
                 sh: Optional[torch.Tensor] = None, albedo: Optional[torch.Tensor] = None,
                 point_lights: Optional[torch.Tensor] = None, visibility: Optional[torch.Tensor] = None,
-                sun_visibility: Optional[torch.Tensor] = None, specular_raster: Optional[torch.Tensor] = None):
+                sun_visibility: Optional[torch.Tensor] = None, specular_raster: Optional[torch.Tensor] = None,
+                brdf: str = "phong"):
         dev = channels.device
         scalars = [x if isinstance(x, torch.Tensor) else torch.tensor(float(x), dtype=torch.float64, device=dev)
                    for x in (light_ambient, specular, shininess)]
@@ -515,7 +520,8 @@ class PhongShadeFunc(torch.autograd.Function):
         sun = sun_visibility.detach().to(torch.float32).contiguous() if sun_visibility is not None else None
         spec = specular_raster.detach().to(torch.float32).contiguous() if specular_raster is not None else None
         image = phong_shade(ch, params, center, bg, sh=shd, albedo=alb, point_lights=pl, visibility=vis,
-                            sun_visibility=sun, specular=spec)
+                            sun_visibility=sun, specular=spec, brdf=brdf)
+        ctx.brdf = brdf
         ctx.save_for_backward(ch, params, center, bg.to(dev, torch.float32), shd, alb, pl, vis, sun, spec)
         ctx.spec_dtype = specular_raster.dtype if specular_raster is not None else None
         ctx.vis_dtype = visibility.dtype if visibility is not None else None
@@ -535,7 +541,7 @@ class PhongShadeFunc(torch.autograd.Function):
         center_grad = ctx.center_is_input and needs[5]
         shaded = phong_shade_backward(ch, params, center, bg, image_b, _scratch_of(ch.device), center_grad=center_grad,
                                       sh=shd, albedo=alb, point_lights=pl, visibility=vis, sun_visibility=sun,
-                                      specular=spec)
+                                      specular=spec, brdf=ctx.brdf)
         spec_b = None
         if spec is not None:
             shaded, spec_b = shaded[:-1], shaded[-1]
@@ -565,6 +571,7 @@ class PhongShadeFunc(torch.autograd.Function):
         out.append(vis_b.to(ctx.vis_dtype) if vis_b is not None and needs[10] else None)
         out.append(sun_b.to(ctx.sun_dtype) if sun_b is not None and needs[11] else None)
         out.append(spec_b.to(ctx.spec_dtype) if spec_b is not None and needs[12] else None)
+        out.append(None)  # brdf
         return tuple(out)
 
 
@@ -921,12 +928,14 @@ class ColoredTriMeshPytorch:
     array) is a tangent-space normal map, read by ``Scene3DPytorch(shading="phong_textured")`` (the model in
     include/deodr_b200.h); the attribute may be reassigned between renders.
 
+    ``metallic_roughness_map`` [Ht,Wt,2] = (roughness_t, metallic_t) (a textured mesh's, likewise; not with a specular
+    map) multiplies the scene's metallic and roughness factors in a ``pbr_textured`` render.
     ``specular_map`` [Ht,Wt,2] (a textured mesh's, likewise) is a specular map whose texel (ks_t, e_t) multiplies the
     scene's specular strength and shininess in a ``phong_textured`` render (the model in include/deodr_b200.h); a tensor
     that may require grad, or an array, and the attribute may be reassigned between renders."""
 
     def __init__(self, faces, vertices, clockwise: bool = False, colors=None, device=None, faces_uv=None, uv=None,
-                 texture=None, normal_map=None, specular_map=None):
+                 texture=None, normal_map=None, specular_map=None, metallic_roughness_map=None):
         self.device = _device(device if device is not None else
                               (vertices.device if isinstance(vertices, torch.Tensor) else None))
         self.faces = np.ascontiguousarray(np.asarray(faces), dtype=np.int64)
@@ -970,6 +979,16 @@ class ColoredTriMeshPytorch:
             if tuple(self.specular_map.shape) != tuple(self.texture.shape[:2]) + (2,):
                 raise ValueError(f"specular_map must be [Ht,Wt,2] with the texture's Ht and Wt = "
                                  f"{tuple(self.texture.shape[:2])}; got {tuple(self.specular_map.shape)}")
+        self.metallic_roughness_map = None
+        if metallic_roughness_map is not None:
+            if not self.textured:
+                raise ValueError("a metallic-roughness map is addressed by the uv: it needs a textured mesh")
+            if specular_map is not None:
+                raise ValueError("a mesh takes a specular map (Phong) or a metallic-roughness map (PBR), not both")
+            self.metallic_roughness_map = self._tensor(metallic_roughness_map)
+            if tuple(self.metallic_roughness_map.shape) != tuple(self.texture.shape[:2]) + (2,):
+                raise ValueError(f"metallic_roughness_map must be [Ht,Wt,2] with the texture's Ht and Wt = "
+                                 f"{tuple(self.texture.shape[:2])}; got {tuple(self.metallic_roughness_map.shape)}")
 
     @property
     def tangents(self) -> VertexTangents:
@@ -1043,6 +1062,10 @@ class Scene3DPytorch:
     a ``specular_map`` adds the map's raster to the same node, and :class:`PhongShadeFunc` reads it per pixel; the map
     receives its gradient.
 
+    ``shading="pbr_textured"`` is the same chain with the metallic-roughness form of :class:`PhongShadeFunc`
+    (``brdf="ggx"``; the model in include/deodr_b200.h): the factors of ``set_material(metallic, roughness)``, which
+    may be tensors that require grad, and a mesh's ``metallic_roughness_map`` rasterised in the specular map's slot.
+
     ``set_point_lights`` adds point lights near the mesh in every shading; a table that requires grad receives its
     gradient, and the vertices receive the lights' share through their normals and their positions.  A flash is a
     light whose position the caller computes from the camera's tensors: its gradient then reaches the camera.  In a
@@ -1054,8 +1077,8 @@ class Scene3DPytorch:
     visibility is a :class:`SunVisibilityFunc`, and a light that requires grad receives the shadow's share."""
 
     def __init__(self, sigma: float = 1.0, backface_culling: bool = True, shading: str = "gouraud"):
-        if shading not in ("gouraud", "phong", "phong_textured"):
-            raise ValueError(f"shading must be 'gouraud', 'phong' or 'phong_textured'; got {shading!r}")
+        if shading not in ("gouraud", "phong", "phong_textured", "pbr_textured"):
+            raise ValueError(f"shading must be 'gouraud', 'phong', 'phong_textured' or 'pbr_textured'; got {shading!r}")
         self.sigma = float(sigma)
         self.backface_culling = bool(backface_culling)
         self.shading = shading
@@ -1071,6 +1094,8 @@ class Scene3DPytorch:
         self._suns: Dict[tuple, SunShadowMap] = {}
         self.specular: Any = 0.0
         self.shininess: Any = 16.0
+        self.metallic: Any = 0.0
+        self.roughness: Any = 0.5
         self.background_color: Optional[np.ndarray] = None
         self._scenes: Dict[tuple, DeviceScene] = {}
         self._phong_scenes: Dict[tuple, DeviceScene] = {}
@@ -1087,10 +1112,23 @@ class Scene3DPytorch:
     def set_specular(self, specular, shininess) -> None:
         """The specular strength ks >= 0 and the shininess e of a Phong render (numbers or 0-d tensors); tensors are
         used as given, so a ``specular`` or ``shininess`` that requires grad receives its gradient."""
+        if self.shading == "pbr_textured":
+            raise ValueError("a 'pbr_textured' render takes set_material(metallic, roughness), not set_specular")
         dev = self.mesh.device if self.mesh is not None else _device(None)
         self.specular, self.shininess = [x if isinstance(x, torch.Tensor) else
                                          torch.tensor(float(x), dtype=torch.float64, device=dev)
                                          for x in (specular, shininess)]
+
+    def set_material(self, metallic, roughness) -> None:
+        """The metallic and roughness factors of a ``pbr_textured`` render (numbers or 0-d tensors); tensors are used
+        as given, so a factor that requires grad receives its gradient."""
+        if self.shading != "pbr_textured":
+            raise ValueError("set_material sets the factors of shading='pbr_textured'; a Phong render takes "
+                             "set_specular")
+        dev = self.mesh.device if self.mesh is not None else _device(None)
+        self.metallic, self.roughness = [x if isinstance(x, torch.Tensor) else
+                                         torch.tensor(float(x), dtype=torch.float64, device=dev)
+                                         for x in (metallic, roughness)]
 
     def set_light(self, light_directional, light_ambient, shadow_map_size: int = 0, shadow_bias: Optional[float] = None,
                   shadow_softness: Optional[float] = None, shadow_bounds=None) -> None:
@@ -1244,13 +1282,20 @@ class Scene3DPytorch:
             channels = torch.cat((channels, vertex_tangents_autograd(m.vertices, uv, m.tangents)), dim=1)
             map_scene = self._albedo_scene(camera, uv, nmap, kind="normal_map")
         smap = spec_scene = None
-        if m.specular_map is not None:
-            # the specular map's raster, after the others
-            smap = m._tensor(m.specular_map)
+        pbr = self.shading == "pbr_textured"
+        if pbr and m.specular_map is not None:
+            raise ValueError("shading='pbr_textured' reads a metallic-roughness map, not a specular map")
+        if not pbr and m.metallic_roughness_map is not None:
+            raise ValueError("a metallic-roughness map needs shading='pbr_textured'")
+        material_map = m.metallic_roughness_map if pbr else m.specular_map
+        if material_map is not None:
+            # the material map's raster (specular or metallic-roughness), after the others
+            kind = "metallic_roughness_map" if pbr else "specular_map"
+            smap = m._tensor(material_map)
             if tuple(smap.shape) != tuple(texture.shape[:2]) + (2,):
-                raise ValueError(f"specular_map must be [Ht,Wt,2] with the texture's Ht and Wt = "
+                raise ValueError(f"{kind} must be [Ht,Wt,2] with the texture's Ht and Wt = "
                                  f"{tuple(texture.shape[:2])}; got {tuple(smap.shape)}")
-            spec_scene = self._albedo_scene(camera, uv, smap, kind="specular_map")
+            spec_scene = self._albedo_scene(camera, uv, smap, kind=kind)
         rasters = 2 + (nmap is not None) + (smap is not None)
         vis = sun = None
         if self.shadow_map_size or self.light_shadow_map_size:
@@ -1270,9 +1315,11 @@ class Scene3DPytorch:
             if nmap is not None:
                 gbuffer = normal_map_autograd(gbuffer, out[2])
         spec = out[rasters - 1] if smap is not None else None
-        return phong_shade_autograd(gbuffer, self.light_directional, self.light_ambient, self.specular,
-                                    self.shininess, camera.center() if camera.is_tensor else camera,
-                                    self.background_color, self.light_sh, albedo, self.point_lights, vis, sun, spec)
+        material = (self.metallic, self.roughness) if pbr else (self.specular, self.shininess)
+        return phong_shade_autograd(gbuffer, self.light_directional, self.light_ambient, material[0], material[1],
+                                    camera.center() if camera.is_tensor else camera, self.background_color,
+                                    self.light_sh, albedo, self.point_lights, vis, sun, spec,
+                                    "ggx" if pbr else "phong")
 
     def _render_phong(self, camera: CameraPytorch) -> torch.Tensor:
         m = self.mesh
@@ -1387,15 +1434,16 @@ class Scene3DPytorch:
         [H,W,C] fp32.  For a textured mesh,
         ``Scene3D.render``'s uv branch: the texture, sampled at the interpolated uv, times the interpolated vertex
         luminosity (differentiable in the vertices, uv, texture and light); with ``shading="phong_textured"`` the
-        sampled texture lit per pixel."""
+        sampled texture lit per pixel, and with ``shading="pbr_textured"`` the metallic-roughness form."""
         if self.mesh is not None and self.mesh.textured:
             if self.shading == "phong":
                 raise ValueError("phong shading of a textured mesh is shading='phong_textured'")
-            if self.shading == "phong_textured":
+            if self.shading in ("phong_textured", "pbr_textured"):
                 return self._render_phong_textured(camera)
             return self._render_textured(camera)
-        if self.shading == "phong_textured":
-            raise ValueError("shading='phong_textured' needs a textured mesh; an untextured one takes shading='phong'")
+        if self.shading in ("phong_textured", "pbr_textured"):
+            raise ValueError(f"shading={self.shading!r} needs a textured mesh; an untextured one takes "
+                             f"shading='phong'")
         if self.mesh is None or self.mesh.vertices_colors is None:
             raise ValueError("render needs a mesh with vertex colours (set_mesh, set_vertices_colors)")
         if self.shading == "phong":

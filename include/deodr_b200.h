@@ -915,6 +915,61 @@ int deodr_b200_phong_shade_specular_map_b(const DeodrPhongIO *io, const float *a
                                           float *albedo_b, float *spec_b, double *sh_b, double *lights_b,
                                           float *vis_b, float *sun_vis_b, double *scratch, void *stream);
 
+/* ---- metallic-roughness materials (textured, GGX) ------------------------------------------------------------------
+ * A per-pixel form for textured views with a separate albedo A [H,W,C] beside the 7-channel G-buffer (N, X, a).  It
+ * reads DeodrPhongIO with its layout unchanged, but params[4] is the metallic factor mf and params[5] the roughness
+ * factor rf (params_b[4..5] their gradients).  An optional metallic-roughness map MR [Ht, Wt, 2] has the albedo
+ * texture's Ht and Wt, is addressed by the same uv / faces_uv and holds (roughness_t, metallic_t) per texel (glTF keeps
+ * them in the G and B channels: slicing them out is the caller's).  The map is rasterised like the albedo, which gives
+ * (R, M) = a x (sample of MR) per pixel.  Per pixel where a != 0:
+ *
+ *   n = N / |N|,  x = X / a,  v = normalize(cam - x),  b_c = A_c / a
+ *   r = rf (R / a),  m = mf (M / a)   (rf and mf without a map; R / a and M / a rounded first)
+ *   alpha = r^2,  F0_c = 0.04 (1 - m) + m b_c
+ *   for each light of unit direction w toward it and intensity E_c:
+ *     directional: w = -l / |l|, E = |l| (grey), times the sun's visibility V when given
+ *     point j:     w = w_j, E_c = I_j[c] / r_j^2, times V_j when given
+ *     nl = <n, w> (the light's term is 0 unless nl > 0), nv = max(0, <n, v>), h = normalize(w + v) (0 when w + v =
+ *     0), nh = max(0, <n, h>), vh = max(0, <v, h>)
+ *     F_c = F0_c + (1 - F0_c) (1 - vh)^5
+ *     S = alpha^2 / (nh^2 (alpha^2 - 1) + 1)^2 / ((nl + sqrt(alpha^2 + (1 - alpha^2) nl^2))
+ *                                                 (nv + sqrt(alpha^2 + (1 - alpha^2) nv^2)))
+ *       (= pi D Vis: GGX D and the separable Smith Vis of glTF 2.0 Appendix B, with pi cancelled)
+ *     term_c = E_c nl [(1 - F_c)(1 - m) A_c + a S F_c]
+ *   image_c = sum over the lights of term_c + (1 - m) A_c (ambient + sh_c(n)) + (1 - a) bg_c
+ *
+ * Conventions.  The clamps are max(0, .) gates that read `> 0`, as the Phong forms'; glTF's |.| differs only where
+ * <n, v> < 0, at the silhouettes of interpolated normals.  Where a = 0 every surface term is 0, with its derivatives,
+ * and the map raster's gradient is 0.  At alpha = 0 the highlight is 0; keeping r > 0 and m in [0, 1] is the caller's
+ * job.  The environment (ambient and SH) lights the diffuse lobe only: there is no specular from the environment.  At
+ * self-occlusion silhouettes front and back surfaces are mixed, as for the Phong form.  A map of ones (R = M = a)
+ * gives the factors-only form bit for bit.
+ *
+ * The adjoint gives A_b (through b_c, F0 too), the G-buffer's (N, X, a) gradients, mr_b = (R_b, M_b), params_b (l,
+ * ambient, mf, rf), lights_b, sh_b, vis_b, sun_vis_b and camera_center_b.  params_b stays a fixed-order sum
+ * (bit-reproducible, no fp64 atomics).
+ *
+ * Limitations: no specular from the environment; bilinear sampling without mip levels; no emissive, occlusion,
+ * clearcoat or anisotropy; textured views only (no per-vertex GGX). */
+
+/* The metallic-roughness shading above with a separate albedo [H,W,C] (required), the map raster mr [H,W,2] = (R, M)
+ * or NULL (the factors alone), an optional environment (sh NULL with sh_channels 0), optional point lights (lights
+ * NULL with nb_lights 0) with their optional visibility vis [H,W,L], and an optional sun visibility sun_vis [H,W].
+ * Refusals, before any launch: DEODR_B200_EINVAL for a NULL io, buffer or albedo, bad sizes or offsets (off_albedo
+ * must be -1), a NULL sh with sh_channels != 0, or a NULL lights with nb_lights != 0 or a vis;
+ * DEODR_B200_EUNSUPPORTED for bad channel or light counts.  No host synchronisation. */
+int deodr_b200_pbr_shade(const DeodrPhongIO *io, const float *albedo, const float *mr, const double *sh,
+                         int sh_channels, const double *lights, int nb_lights, int light_channels, const float *vis,
+                         const float *sun_vis, void *stream);
+/* Its adjoint from io->image_b: channels_b [H,W,7], albedo_b [H,W,C], mr_b [H,W,2] (with mr), params_b and
+ * camera_center_b (when given) overwritten, and with the optional inputs sh_b, lights_b, vis_b and sun_vis_b.  Same
+ * refusals, plus DEODR_B200_EINVAL for a NULL image_b, channels_b, params_b, albedo_b or scratch, an mr_b that is
+ * non-NULL exactly when mr is not, or a NULL gradient of a given optional input. */
+int deodr_b200_pbr_shade_b(const DeodrPhongIO *io, const float *albedo, const float *mr, const double *sh,
+                           int sh_channels, const double *lights, int nb_lights, int light_channels, const float *vis,
+                           const float *sun_vis, float *albedo_b, float *mr_b, double *sh_b, double *lights_b,
+                           float *vis_b, float *sun_vis_b, double *scratch, void *stream);
+
 /* One parameter vector of a heavy-ball update (device pointers, `size` entries each):
  *   step = clamp(-grad * factor, -max_step, max_step)   (max_step = INFINITY: unclamped)
  *   speed = (1 - damping) (speed * inertia + (1 - inertia) step);  value += speed
