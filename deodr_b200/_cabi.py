@@ -247,6 +247,14 @@ class HostScene(C.Structure):
     ]
 
 
+class CollisionMesh(C.Structure):
+    """``DeodrCollisionMesh``: the device arrays of the self-collision entry points."""
+
+    _fields_ = [(name, C.c_void_p) for name in ("faces", "edges", "neighbour_offset", "neighbour_index",
+                                                 "corner_offset", "corner_index", "end_offset", "end_index")] + [
+        ("nb_faces", C.c_int32), ("nb_edges", C.c_int32), ("nb_vertices", C.c_int32)]
+
+
 # every symbol include/deodr_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("deodr_b200_workspace_create", C.c_int, [C.POINTER(C.c_void_p), C.c_int]),
@@ -407,6 +415,12 @@ SYMBOLS = [
      [C.POINTER(LoopLevel), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("deodr_b200_loop_subdivide_b", C.c_int,
      [C.POINTER(LoopLevel), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_self_collision", C.c_int,
+     [C.c_void_p, C.POINTER(CollisionMesh), C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p,
+      C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_self_intersections", C.c_int,
+     [C.c_void_p, C.POINTER(CollisionMesh), C.c_void_p, C.c_double, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
+      C.c_void_p]),
     ("deodr_b200_render_host", C.c_int,
      [C.c_void_p, C.POINTER(HostScene), C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p]),
     ("deodr_b200_render_b_host", C.c_int,

@@ -1646,6 +1646,7 @@ void deodr_b200_workspace_destroy(DeodrWorkspace *ws) {
                       &ws->h_grads, &ws->h_obs, &ws->h_err, &ws->h_err_b};
     for (DevBuf *b : bufs) b->release();
     deodr_host_path_destroy(ws);
+    deodr_collision_destroy(ws);
     if (ws->host_scratch) cudaFreeHost(ws->host_scratch);
     for (cudaEvent_t e : ws->ev_start) cudaEventDestroy(e);
     for (cudaEvent_t e : ws->ev_stop) cudaEventDestroy(e);

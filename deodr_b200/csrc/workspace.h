@@ -169,9 +169,11 @@ struct DeodrWorkspace {
     DevBuf h_faces, h_faces_uv, h_ij, h_depths, h_uv, h_colors, h_shade, h_edgeflags, h_textured, h_shaded, h_texture,
         h_background, h_image, h_z, h_owner, h_image_b, h_grads, h_obs, h_err, h_err_b;
     struct HostPath *host = nullptr;  // pinned staging, copy threads, cache of the last host forward (host_api.cu)
+    struct CollisionState *collision = nullptr;  // self-collision plan and buffers (collision.cu)
 };
 
 void deodr_host_path_destroy(DeodrWorkspace *ws);  // host_api.cu
+void deodr_collision_destroy(DeodrWorkspace *ws);  // collision.cu
 
 // forward pass of one view into slot 0 with optional on-device index validation (checkSceneValid, DR.h:2703-2714);
 // always verified before it returns (the host path synchronises anyway)

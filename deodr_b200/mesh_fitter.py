@@ -6,7 +6,9 @@ A step centres the vertices, applies the rigid pose, renders (depth or colour), 
 back-propagates through the render and the pose, adds the gradient of the Laplacian rigidity energy and takes clamped
 heavy-ball steps - every part on the GPU: the renderer and the scene ops (mesh_ops.py), and for the fitter's own maths
 the kernels of csrc/fitter.cu (include/deodr_b200.h, "mesh fitting").  Nothing is read back to the host inside
-``step()`` apart from the renderer's own verdict; its energy is a 0-d fp64 CUDA tensor.
+``step()`` apart from the renderer's own verdict (and, with ``cself > 0``, the self-collision's); its energy is a 0-d
+fp64 CUDA tensor.  With ``cself > 0`` the step adds ``DeviceSelfCollisionEnergy`` of the un-posed vertices to the
+rigidity's gradient and energy; ``energy_self_collision`` holds its energy.
 """
 
 from __future__ import annotations
@@ -40,13 +42,9 @@ def euler_to_quaternion(euler) -> np.ndarray:
     return Rotation.from_euler("zyx", np.asarray(euler, dtype=np.float64)).as_quat()
 
 
-def laplacian_neighbours(faces, nb_vertices: int) -> Tuple[np.ndarray, np.ndarray]:
-    """Neighbour CSR (offset [V+1], index) int32 of the "shares a face" adjacency, itself excluded, neighbours ascending:
-    the matrix A of the Laplacian L = D - A.  Raises ValueError for a mesh with more than one connected component
-    (a vertex in no face is a component of its own), where the rigidity energy leaves a component free to drift."""
-    from scipy.sparse import coo_matrix
-    from scipy.sparse.csgraph import connected_components
-
+def edge_neighbours(faces, nb_vertices: int) -> Tuple[np.ndarray, np.ndarray]:
+    """Neighbour CSR (offset [V+1], index) int32 of the "shares a face" adjacency, itself excluded, neighbours
+    ascending: the matrix A of the Laplacian L = D - A, and the one-ring of the self-collision exclusion."""
     arr = topology_arrays(faces, nb_vertices)
     V = arr["nb_vertices"]
     faces = np.asarray(arr["faces"]).view(np.uint32).astype(np.int64)
@@ -62,8 +60,19 @@ def laplacian_neighbours(faces, nb_vertices: int) -> Tuple[np.ndarray, np.ndarra
     rows, cols = rows[order], cols[order]
     offset = np.zeros(V + 1, dtype=np.int32)
     np.cumsum(np.bincount(rows, minlength=V), out=offset[1:])
-    index = cols.astype(np.int32)
-    n_components, _ = connected_components(coo_matrix((np.ones(rows.size), (rows, cols)), shape=(V, V)), directed=False)
+    return offset, cols.astype(np.int32)
+
+
+def laplacian_neighbours(faces, nb_vertices: int) -> Tuple[np.ndarray, np.ndarray]:
+    """:func:`edge_neighbours`, for a mesh of one connected component: raises ValueError for more (a vertex in no face
+    is a component of its own), where the rigidity energy leaves a component free to drift."""
+    from scipy.sparse import csr_matrix
+    from scipy.sparse.csgraph import connected_components
+
+    offset, index = edge_neighbours(faces, nb_vertices)
+    V = offset.size - 1
+    adjacency = csr_matrix((np.ones(index.size), index, offset), shape=(V, V))
+    n_components, _ = connected_components(adjacency, directed=False)
     if n_components > 1:
         raise ValueError(f"the mesh has {n_components} connected components; the Laplacian rigidity energy needs one")
     return offset, index
@@ -218,6 +227,102 @@ class DeviceLaplacianRigidEnergy:
         return energy, grad
 
 
+def collision_mesh_arrays(faces, nb_vertices: int) -> dict:
+    """Host arrays of ``DeodrCollisionMesh`` (numpy int32): the faces, the unique undirected edges (lo, hi) ordered by
+    (lo, hi) - the edge order of :func:`topology_arrays` -, the one-ring CSR of :func:`edge_neighbours`, and the
+    corners 3f + k and edge ends 2e + j of every vertex as CSR, ascending.  Face indices are checked here."""
+    arr = topology_arrays(faces, nb_vertices)
+    V = arr["nb_vertices"]
+    f = np.asarray(arr["faces"]).view(np.uint32).astype(np.int64)
+    a = f.reshape(-1)
+    b = f[:, [1, 2, 0]].reshape(-1)
+    key = np.unique(np.minimum(a, b) * V + np.maximum(a, b))
+    edges = np.stack((key // V, key % V), axis=1)
+    offset, index = edge_neighbours(faces, V)
+
+    def csr(flat):
+        off = np.zeros(V + 1, dtype=np.int32)
+        np.cumsum(np.bincount(flat, minlength=V), out=off[1:])
+        return off, np.argsort(flat, kind="stable").astype(np.int32)
+
+    corner_offset, corner_index = csr(a)
+    end_offset, end_index = csr(edges.reshape(-1))
+    return {"faces": arr["faces"], "edges": np.ascontiguousarray(edges, dtype=np.int32), "neighbour_offset": offset,
+            "neighbour_index": index if index.size else np.zeros(1, np.int32), "corner_offset": corner_offset,
+            "corner_index": corner_index, "end_offset": end_offset, "end_index": end_index,
+            "nb_faces": arr["nb_faces"], "nb_edges": int(edges.shape[0]), "nb_vertices": V}
+
+
+class DeviceSelfCollisionEnergy:
+    """A self-collision penalty on the device (include/deodr_b200.h, "Self-collision"): for thickness delta and weight
+    w, E = w sum phi(d) over the vertex-triangle and edge-edge pairs outside each other's one-ring, with
+    phi(d) = (delta - d)^2 below delta.  ``evaluate(vertices)`` -> (energy 0-d f64, grad [V,3] f64); ``min_distance``
+    (0-d) is the smallest such distance of the last evaluation, or delta when there is none; ``intersections`` lists the
+    face pairs that cross.  ``vertices_ref`` only sizes the grid's cells (their median edge length, at least delta).
+    Meshes of several connected components are accepted.  Each call reads one word back from the device."""
+
+    def __init__(self, faces, vertices_ref, thickness: float, weight: float, device="cuda"):
+        from .renderer import default_renderer
+
+        self.device = torch.device(device)
+        vertices_ref = np.asarray(vertices_ref, dtype=np.float64)
+        self.thickness, self.weight = float(thickness), float(weight)
+        arrays = collision_mesh_arrays(faces, vertices_ref.shape[0])
+        self.nb_vertices, self.nb_faces = arrays["nb_vertices"], arrays["nb_faces"]
+        self.t = {k: torch.from_numpy(np.ascontiguousarray(v)).to(self.device) for k, v in arrays.items()
+                  if isinstance(v, np.ndarray)}
+        self._mesh = _cabi.CollisionMesh()
+        for name, t in self.t.items():
+            setattr(self._mesh, name, t.data_ptr())
+        self._mesh.nb_faces, self._mesh.nb_edges, self._mesh.nb_vertices = (arrays["nb_faces"], arrays["nb_edges"],
+                                                                            arrays["nb_vertices"])
+        e = arrays["edges"]
+        lengths = np.linalg.norm(vertices_ref[e[:, 0]] - vertices_ref[e[:, 1]], axis=1)
+        self.cell_size = max(float(np.median(lengths)) if lengths.size else 0.0, self.thickness)
+        self.min_distance = torch.empty((), dtype=torch.float64, device=self.device)
+        self._renderer = default_renderer(self.device.index if self.device.index is not None else None)
+        self._pairs = torch.empty((max(16, self.nb_faces // 8), 2), dtype=torch.int32, device=self.device)
+
+    def _vertices(self, vertices: torch.Tensor) -> torch.Tensor:
+        if tuple(vertices.shape) != (self.nb_vertices, 3):
+            raise ValueError(f"vertices must be [{self.nb_vertices},3]; got {tuple(vertices.shape)}")
+        return _f64(vertices, self.device)
+
+    def evaluate(self, vertices: torch.Tensor, grad: Optional[torch.Tensor] = None,
+                 energy: Optional[torch.Tensor] = None,
+                 add_to: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """-> (energy, grad): grad = add_to + dE/dvertices (``add_to`` may be ``grad`` itself, to add in place)."""
+        vertices = self._vertices(vertices)
+        if grad is None:
+            grad = torch.empty((self.nb_vertices, 3), dtype=torch.float64, device=self.device)
+        if energy is None:
+            energy = torch.empty((), dtype=torch.float64, device=self.device)
+        r = self._renderer
+        with r._lock:
+            _cabi.check(r.lib.deodr_b200_self_collision(
+                r._ws, C.byref(self._mesh), vertices.data_ptr(), self.thickness, self.weight, self.cell_size,
+                _ptr(add_to), grad.data_ptr(), energy.data_ptr(), self.min_distance.data_ptr(), _stream(self.device)))
+        return energy, grad
+
+    def intersections(self, vertices: torch.Tensor) -> torch.Tensor:
+        """The face pairs (i < j) that share no vertex and where an edge of one properly crosses the other: [P,2]
+        int64, sorted.  Coplanar and touching contacts are not reported."""
+        vertices = self._vertices(vertices)
+        r = self._renderer
+        count = C.c_int64(0)
+        for _ in range(2):
+            with r._lock:
+                _cabi.check(r.lib.deodr_b200_self_intersections(
+                    r._ws, C.byref(self._mesh), vertices.data_ptr(), self.cell_size, self._pairs.data_ptr(),
+                    self._pairs.shape[0], C.byref(count), _stream(self.device)))
+            if count.value <= self._pairs.shape[0]:
+                break
+            self._pairs = torch.empty((count.value + count.value // 4, 2), dtype=torch.int32, device=self.device)
+        pairs = self._pairs[:count.value].to(torch.int64)
+        order = torch.argsort(pairs[:, 0] * self.nb_faces + pairs[:, 1])
+        return pairs[order]
+
+
 def fitter_camera(camera_center, width: int, height: int, focal=None, distortion=None) -> CameraParams:
     """The camera of the reference fitters' ``set_image``: rotation diag(1, -1, -1), centre ``camera_center``, focal
     ``2 * width`` by default, principal point at the image centre."""
@@ -232,13 +337,25 @@ def fitter_camera(camera_center, width: int, height: int, focal=None, distortion
 class _PoseFitter:
     """State and update rule shared by the two fitters: vertices, quaternion and translation with their speeds."""
 
-    def _init_pose(self, vertices, faces, euler_init, translation_init, cregu, inertia, damping, device):
+    def _init_pose(self, vertices, faces, euler_init, translation_init, cregu, inertia, damping, device, cself=0.0,
+                   self_collision_thickness=None):
         self.device = torch.device(device)
         self.cregu, self.inertia, self.damping = cregu, inertia, damping
         self.faces = np.ascontiguousarray(np.asarray(faces), dtype=np.int64)
         self.vertices_init = np.array(vertices, dtype=np.float64)
         self.nb_vertices = self.vertices_init.shape[0]
         self.rigid_energy = DeviceLaplacianRigidEnergy(self.faces, self.vertices_init, cregu, self.device)
+        # the self-collision term, evaluated at the un-posed vertices (the pose is rigid: distances do not change)
+        self.cself = float(cself)
+        self.self_collision = None
+        self.energy_self_collision = torch.zeros((), dtype=torch.float64, device=self.device)
+        if self.cself < 0:
+            raise ValueError(f"cself must be >= 0; got {cself}")
+        if self.cself > 0:
+            if self_collision_thickness is None:
+                raise ValueError("cself > 0 needs self_collision_thickness")
+            self.self_collision = DeviceSelfCollisionEnergy(self.faces, self.vertices_init, self_collision_thickness,
+                                                            self.cself, self.device)
         self._scratch = new_scratch(self.device)
         self.view: Optional[DeviceMeshView] = None
         self.set_mesh_transform_init(euler=euler_init, translation=translation_init)
@@ -272,6 +389,15 @@ class _PoseFitter:
         self.iter = 0
         return fitter_camera(self.camera_center, self.width, self.height, focal, distortion)
 
+    def _regularisers(self) -> None:
+        """The rigidity's gradient and energy into ``_grad_rigid`` and ``_energy_rigid``, plus the self-collision's
+        when ``cself > 0`` (then also in ``energy_self_collision``)."""
+        self.rigid_energy.evaluate(self.vertices, grad=self._grad_rigid, energy=self._energy_rigid)
+        if self.self_collision is not None:
+            self.self_collision.evaluate(self.vertices, grad=self._grad_rigid, energy=self.energy_self_collision,
+                                         add_to=self._grad_rigid)
+            self._energy_rigid += self.energy_self_collision
+
     def _render_pose(self) -> torch.Tensor:
         return pose(self.vertices, self.transform_quaternion, self.transform_translation, self._scratch,
                     out=self._transformed)
@@ -280,7 +406,7 @@ class _PoseFitter:
                                     extra_params=()) -> torch.Tensor:
         pose_backward(self.vertices, self.transform_quaternion, transformed_b, self._scratch,
                       out=(self._vertices_b, self.transform_quaternion_b, self.transform_translation_b))
-        self.rigid_energy.evaluate(self.vertices, grad=self._grad_rigid, energy=self._energy_rigid)
+        self._regularisers()
         energy = torch.empty((), dtype=torch.float64, device=self.device)
         params = [heavy_ball(self.transform_quaternion, self.speed_quaternion, self.transform_quaternion_b,
                              self.step_factor_quaternion, self.step_max_quaternion, normalize=True),
@@ -298,7 +424,8 @@ class MeshDepthFitter(_PoseFitter):
     ``step()`` -> (energy 0-d f64, depth [H,W] f64 clipped to [0, max_depth], diff_image [H,W] f64), CUDA tensors."""
 
     def __init__(self, vertices, faces, euler_init, translation_init, cregu: float = 2000, inertia: float = 0.96,
-                 damping: float = 0.05, device="cuda"):
+                 damping: float = 0.05, device="cuda", cself: float = 0.0,
+                 self_collision_thickness: Optional[float] = None):
         self.step_factor_vertices = 0.0005
         self.step_max_vertices = 1
         self.step_factor_quaternion = 0.00006
@@ -311,7 +438,8 @@ class MeshDepthFitter(_PoseFitter):
         self.camera_center = object_center + np.array([-0.5, 0, 5]) * object_radius
         self.max_depth = None
         self.depth_scale = 1.0
-        self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device)
+        self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device, cself,
+                        self_collision_thickness)
         self.reset()
 
     def reset(self) -> None:
@@ -356,7 +484,8 @@ class MeshRGBFitterWithPose(_PoseFitter):
 
     def __init__(self, vertices, faces, euler_init, translation_init, default_color, default_light_directional,
                  default_light_ambient: float, cregu: float = 2000, inertia: float = 0.96, damping: float = 0.05,
-                 update_lights: bool = True, update_color: bool = True, device="cuda"):
+                 update_lights: bool = True, update_color: bool = True, device="cuda",
+                 cself: float = 0.0, self_collision_thickness: Optional[float] = None):
         self.step_factor_vertices = 0.0005
         self.step_max_vertices = 0.5
         self.step_factor_quaternion = 0.00006
@@ -374,7 +503,8 @@ class MeshRGBFitterWithPose(_PoseFitter):
         self.camera_center = object_center + np.array([0, 0, 9]) * object_radius
         self.background_color = None
         self.sigma = 1.0
-        self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device)
+        self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device, cself,
+                        self_collision_thickness)
         self.reset()
 
     def reset(self) -> None:
@@ -459,7 +589,8 @@ class MeshRGBFitterWithPoseMultiFrame(_PoseFitter):
 
     def __init__(self, vertices, faces, euler_init, translation_init, default_color, default_light_directional,
                  default_light_ambient: float, cregu: float = 2000, cdata: float = 1, inertia: float = 0.97,
-                 damping: float = 0.15, update_lights: bool = True, update_color: bool = True, device="cuda"):
+                 damping: float = 0.15, update_lights: bool = True, update_color: bool = True, device="cuda",
+                 cself: float = 0.0, self_collision_thickness: Optional[float] = None):
         self.step_factor_vertices = 0.0005
         self.step_max_vertices = 0.5
         self.step_factor_quaternion = 0.00005
@@ -479,7 +610,8 @@ class MeshRGBFitterWithPoseMultiFrame(_PoseFitter):
         self.background_color = None
         self.sigma = 1.0
         self.scenes = None
-        self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device)
+        self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device, cself,
+                        self_collision_thickness)
         self.reset()
 
     def set_mesh_transform_init(self, euler, translation) -> None:
@@ -657,7 +789,7 @@ class MeshRGBFitterWithPoseMultiFrame(_PoseFitter):
         pose_frames_backward(self.vertices, self.transform_quaternion, transformed_b, self._scratch,
                              center=self.iter < 500, scale=coef, losses=self._losses, energy_data=self._energy_data,
                              out=(self._vertices_b, self.transform_quaternion_b, self.transform_translation_b))
-        self.rigid_energy.evaluate(self.vertices, grad=self._grad_rigid, energy=self._energy_rigid)
+        self._regularisers()
         energy = torch.empty((), dtype=torch.float64, device=self.device)
         params = [heavy_ball(self.transform_quaternion, self.speed_quaternion, self.transform_quaternion_b,
                              self.step_factor_quaternion, self.step_max_quaternion, normalize=True),

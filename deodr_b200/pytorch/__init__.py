@@ -28,5 +28,7 @@ from .scene3d_pytorch import (  # noqa: F401
     RenderMesh2DTexturedFunc,
     RigidEnergyFunc,
     Scene3DPytorch,
+    SelfCollisionEnergyFunc,
+    SelfCollisionEnergyPytorch,
     VertexNormalsFunc,
 )

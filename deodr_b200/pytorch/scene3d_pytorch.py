@@ -23,6 +23,7 @@ caller may add terms of its own to the loss or step the parameters with ``torch.
                            gradients to ij, uv, shade and texture (a textured mesh: Scene3D.render's uv branch)
     PoseFunc              (vertices, quaternion [4], translation [3]) -> qrot(q / |q|, v - mean v) + t
     RigidEnergyFunc        (vertices, DeviceLaplacianRigidEnergy) -> energy 0-d
+    SelfCollisionEnergyFunc (vertices, DeviceSelfCollisionEnergy) -> energy 0-d
     LoopSubdivisionFunc    (vertices [V,3], colors [V,C] | None, LoopSubdivision) -> (fine vertices, fine colours)
                            the reference's Loop subdivision (ColoredTriMeshPytorch.subdivise), its transpose backward
     PhongShadeFunc         (channels [H,W,C+7], light_directional [3] | None, light_ambient, specular, shininess,
@@ -68,7 +69,7 @@ from typing import Any, Dict, Optional, Tuple
 import numpy as np
 import torch
 
-from ..mesh_fitter import DeviceLaplacianRigidEnergy, new_scratch, pose, pose_backward
+from ..mesh_fitter import DeviceLaplacianRigidEnergy, DeviceSelfCollisionEnergy, new_scratch, pose, pose_backward
 from ..mesh_ops import (CameraParams, LoopSubdivision, MeshTopology, camera_center, lit_vertex_colors,
                         ShadowCubes, SunShadowMap, check_shadow_arguments, check_sun_shadow_arguments,
                         cube_project_backward, lit_vertex_colors_backward, sun_project_backward, sun_visibility,
@@ -448,6 +449,23 @@ class RigidEnergyFunc(torch.autograd.Function):
     def backward(ctx: Any, energy_b: Optional[torch.Tensor], grad_b: Optional[torch.Tensor]):  # type: ignore
         if energy_b is None:
             return None, None
+        (grad,) = ctx.saved_tensors
+        return (energy_b * grad).to(ctx.dtype), None
+
+
+class SelfCollisionEnergyFunc(torch.autograd.Function):
+    """(vertices [V,3], DeviceSelfCollisionEnergy) -> energy 0-d fp64; the backward is ``energy_b * grad`` with the
+    gradient of the same evaluation."""
+
+    @staticmethod
+    def forward(ctx: Any, vertices: torch.Tensor, model: DeviceSelfCollisionEnergy):  # type: ignore
+        energy, grad = model.evaluate(_f64(vertices))
+        ctx.save_for_backward(grad)
+        ctx.dtype = vertices.dtype
+        return energy
+
+    @staticmethod
+    def backward(ctx: Any, energy_b: torch.Tensor):  # type: ignore
         (grad,) = ctx.saved_tensors
         return (energy_b * grad).to(ctx.dtype), None
 
@@ -1500,3 +1518,30 @@ class LaplacianRigidEnergyPytorch:
             return energy, grad, None
         energy, grad = self.model.evaluate(vertices)
         return energy, grad, None
+
+
+class SelfCollisionEnergyPytorch:
+    """A self-collision penalty under autograd (``DeviceSelfCollisionEnergy``): ``evaluate(v)`` -> energy 0-d fp64,
+    differentiable when ``v`` requires grad.  ``min_distance`` and ``intersections(v)`` are the device model's."""
+
+    def __init__(self, faces, vertices_ref, thickness: float, weight: float, device=None):
+        faces = faces.faces if hasattr(faces, "faces") else faces
+        if isinstance(faces, torch.Tensor):
+            faces = faces.cpu().numpy()
+        if isinstance(vertices_ref, torch.Tensor):
+            device = vertices_ref.device if device is None else device
+            vertices_ref = vertices_ref.detach().cpu().numpy()
+        self.model = DeviceSelfCollisionEnergy(np.asarray(faces), np.asarray(vertices_ref, dtype=np.float64), thickness,
+                                               weight, _device(device))
+
+    @property
+    def min_distance(self) -> torch.Tensor:
+        return self.model.min_distance
+
+    def intersections(self, vertices: torch.Tensor) -> torch.Tensor:
+        return self.model.intersections(vertices.detach())
+
+    def evaluate(self, vertices: torch.Tensor) -> torch.Tensor:
+        if vertices.requires_grad:
+            return SelfCollisionEnergyFunc.apply(vertices, self.model)
+        return self.model.evaluate(vertices)[0]

@@ -1057,6 +1057,65 @@ int deodr_b200_loop_subdivide_b(const DeodrLoopLevel *level, const double *fine_
                                 const double *fine_colors_b, int nb_colors, double *vertices_b, double *colors_b,
                                 void *stream);
 
+/* ---- Self-collision: a penalty that keeps a mesh from passing through itself, and a self-intersection query, in fp64
+ * on device buffers (csrc/collision.cu).  For a mesh with faces [F,3], vertices [V,3], thickness delta > 0, weight w >= 0:
+ *   E = w sum_{(v,t) in P_vt} phi(d(v,t)) + w sum_{{e,e'} in P_ee} phi(d(e,e')),  phi(d) = (delta - d)^2 if d < delta else 0
+ * d(v,t) is the distance from a vertex to a closed triangle (Ericson, Real-Time Collision Detection 5.1.5,
+ * ClosestPtPointTriangle), d(e,e') the distance between two closed segments, the mesh's unique undirected edges
+ * (ClosestPtSegmentSegment, 5.1.9, with EPSILON = 0: its clamping order and its parallel case, s = 0 when
+ * a e - b^2 = 0; the pair is evaluated with the lower edge id as the first segment).
+ * Excluded pairs (the one-ring): (v,t) when v is a corner of t or an edge neighbour of a corner; {e,e'} when an
+ * endpoint of one equals an endpoint of the other or is an edge neighbour of one.  A vertex in no face takes no part;
+ * a face whose cross(b - a, c - a) is exactly zero takes part in no (v,t) pair, its edges still do.
+ * Gradients from the closest points (envelope theorem), with c = 2 w (delta - d):
+ *   (v,t): q = sum_i w_i a_i, n = (p - q) / d:   dE/dp = -c n,  dE/da_i = +c w_i n
+ *   {e,e'}: c1 = p1 + s (q1 - p1), c2 = p2 + t (q2 - p2), n = (c1 - c2) / d:  p1, q1 get -c (1 - s) n, -c s n;
+ *           p2, q2 get +c (1 - t) n, +c t n
+ * A pair at d = 0 adds w delta^2 to E and nothing to the gradient.  *min_distance is the smallest d over the pairs
+ * closer than delta, or delta when there is none.  A non-finite vertex coordinate (of a vertex in a face) makes
+ * *energy and *min_distance NaN; the primitives that touch it are left out of the grid.
+ * The distances use no fused multiply-add: each product and sum is rounded as the fp64 restatement
+ * (tests/self_collision_ref.py) rounds it, so every d equals the restatement's bit for bit. */
+typedef struct DeodrCollisionMesh {
+    const uint32_t *faces;            /* [F,3] */
+    const int32_t *edges;             /* [E,2] the unique undirected edges (lo, hi), lo <= hi, ordered by (lo, hi) */
+    const int32_t *neighbour_offset;  /* [V+1] CSR: the edge neighbours of every vertex, itself excluded ... */
+    const int32_t *neighbour_index;   /* ... ascending in every row (they are binary-searched) */
+    const int32_t *corner_offset;     /* [V+1] CSR: the corners 3 f + k of every vertex, ascending ... */
+    const int32_t *corner_index;      /* ... (length 3F) */
+    const int32_t *end_offset;        /* [V+1] CSR: the edge ends 2 e + j of every vertex, ascending ... */
+    const int32_t *end_index;         /* ... (length 2E) */
+    int32_t nb_faces, nb_edges, nb_vertices;
+} DeodrCollisionMesh;
+
+/* E, its gradient and the minimum distance.  grad [V,3] = grad_in + dE/dvertices (grad_in may be NULL, or equal to
+ * grad to add in place); *energy and *min_distance are device scalars.  Broad phase: a uniform grid of cells of
+ * max(cell_size, thickness) (grown when the grid would exceed 2^21 cells or 1024 per axis), over the bounding box of
+ * the finite vertices.  Every (cell, primitive) entry is sorted by a stable radix sort; the vertex-triangle pairs are
+ * found from both sides and the edge-edge pairs once per edge at the first cell the two edges share.  The gradient is
+ * gathered per vertex in CSR order and the sums are fixed-order grid reductions: no fp64 atomics, two calls on the same
+ * input give the same bits.  The workspace keeps the entry capacity of the previous call: the call reads one word,
+ * the entry count, from pinned memory after the grid is built and, when it exceeds the capacity, grows it and runs
+ * again (the first call builds the plan this way).  Nothing else is read back.  Face indices are not checked here:
+ * the host checks them where it builds the topology.  EINVAL for a NULL ws, mesh, array, vertices, grad, energy or
+ * min_distance, an empty mesh, thickness <= 0 or non-finite, weight < 0 or non-finite, or a non-finite cell_size;
+ * EUNSUPPORTED when the grid would need 2^31 entries or more. */
+int deodr_b200_self_collision(DeodrWorkspace *ws, const DeodrCollisionMesh *mesh, const double *vertices,
+                              double thickness, double weight, double cell_size, const double *grad_in, double *grad,
+                              double *energy, double *min_distance, void *stream);
+
+/* The face pairs (i < j) that share no vertex and where an edge of one properly crosses the other: the edge (p, q)
+ * and the triangle (a, b, c) with O(x, y, z, w) = dot(cross(y - x, z - x), w - x) have O(a,b,c,p) and O(a,b,c,q) of
+ * strictly opposite signs, and O(p,q,a,b), O(p,q,b,c), O(p,q,c,a) of the same non-zero sign.  Coplanar contacts and
+ * touching contacts (a zero orientation) are not reported.  Faces that share a vertex are never paired.  Same
+ * products and sums as the restatement, no fused multiply-add, so the signs are the restatement's bit for bit.
+ * Writes up to `capacity` pairs to pairs [capacity,2] (int32, in an order fixed by the grid) and their number to
+ * *count (host); when *count > capacity, call again with a buffer of *count pairs.  Grid as above with cells of
+ * cell_size and the faces' bounding boxes; one read-back of the entry and pair counts.  Same refusals, with
+ * cell_size > 0 and finite, and a NULL count (or a NULL pairs with capacity > 0). */
+int deodr_b200_self_intersections(DeodrWorkspace *ws, const DeodrCollisionMesh *mesh, const double *vertices,
+                                  double cell_size, int32_t *pairs, int64_t capacity, int64_t *count, void *stream);
+
 /* Per-kernel device timing with CUDA events recorded on the launching stream (for bench.py's roofline).
  * enable: pre-creates `max_records` event pairs (0 disables and frees them).  Every instrumented launch group of the
  * following render / render_b calls then records one (phase, start, stop) triple until the pool is exhausted.
