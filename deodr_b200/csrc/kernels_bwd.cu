@@ -8,6 +8,61 @@
 #include <cstdlib>
 #include <cstring>
 
+// -DDEODR_SMALLBWD_PHASE_CLOCKS (measurement builds only, scripts/small_bwd_phases.py): every thread of k_small_tri_bwd
+// adds the clock64() cycles it spent in each phase of small_triangle_adjoint (phases.h: SB_*) to g_smallbwd_clocks,
+// summed per warp first; the slots after the phases count the threads and the threads that own no pixel (hidden
+// triangles), and g_smallbwd_hist counts the threads by pixels owned (0..64, before the edge-tile masking).  Read back
+// (and cleared) with deodr_b200_small_bwd_phase_clocks.
+#ifdef DEODR_SMALLBWD_PHASE_CLOCKS
+constexpr int SB_SLOTS = 5 + 2;  // SB_PHASES, threads, hidden
+constexpr int SB_HIST = 65;
+__device__ unsigned long long g_smallbwd_clocks[SB_SLOTS];
+__device__ unsigned int g_smallbwd_hist[SB_HIST];
+struct SmallBwdClocks {
+    unsigned int acc[5];
+    int owned;
+    long long prev;
+    __host__ __device__ SmallBwdClocks() : acc{}, owned(0), prev(0) {
+#if defined(__CUDA_ARCH__)
+        prev = clock64();
+#endif
+    }
+    __host__ __device__ void lap(int phase) {
+#if defined(__CUDA_ARCH__)
+        const long long now = clock64();
+        acc[phase] += (unsigned int)(now - prev);
+        prev = now;
+#endif
+    }
+    __host__ __device__ void set_owned(unsigned long long mine) {
+#if defined(__CUDA_ARCH__)
+        owned = __popcll(mine);
+#endif
+    }
+    __host__ __device__ void done() const {
+#if defined(__CUDA_ARCH__)
+        const unsigned int m = __activemask(), leader = __ffs(m) - 1, lane = threadIdx.x & 31;
+#pragma unroll
+        for (int k = 0; k < 5; k++) {
+            const unsigned int v = __reduce_add_sync(m, acc[k]);
+            if (lane == leader) atomicAdd(&g_smallbwd_clocks[k], (unsigned long long)v);
+        }
+        const unsigned int hidden = __popc(__ballot_sync(m, owned == 0));
+        if (lane == leader) {
+            atomicAdd(&g_smallbwd_clocks[5], (unsigned long long)__popc(m));
+            atomicAdd(&g_smallbwd_clocks[6], (unsigned long long)hidden);
+        }
+        const unsigned int same = __match_any_sync(m, owned);
+        if (lane == (unsigned int)(__ffs(same) - 1)) atomicAdd(&g_smallbwd_hist[owned], (unsigned int)__popc(same));
+#endif
+    }
+};
+#define SMALLBWD_START SmallBwdClocks sb_clocks_
+#define SMALLBWD_LAP(phase) sb_clocks_.lap(phase)
+#define SMALLBWD_OWNED(mine) sb_clocks_.set_owned(mine)
+#define SMALLBWD_DONE sb_clocks_.done()
+#endif
+
 #include "kernels_common.cuh"
 
 // antialiase_error adjoint, pixels outside every edge band: image_b = -2 (obs - image) err_b (DR.h:3054-3060), consumed
@@ -350,8 +405,8 @@ template <int MAXC>
 static void launch_bwd(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const SceneView &s, const DeodrViewIO &io,
                        double sigma, int flags, const DeodrGrads &g, const DeodrBackgroundGrads &bg) {
     // Three independent chains (disjoint pixel sets, all accumulate with atomics): edge tiles (longest tail: launched
-    // first, on the lane's high-priority stream, so that its CTAs are dispatched first), tiles with large triangles,
-    // small triangles.  On an equal-priority stream the edge chain's CTAs were dispatched last in a graph replay: on the
+    // first, on the lane's high-priority stream, so that its CTAs are dispatched first), small triangles (the longest
+    // kernel: launched next), tiles with large triangles.  On an equal-priority stream the edge chain's CTAs were dispatched last in a graph replay: on the
     // 1M-triangle scene k_raster_bwd started 76 us after the adjoint began, and k_finalize_edges ran alone at the end.
     cudaStream_t st = lane.main;
     bool first = true;
@@ -406,9 +461,32 @@ static void launch_bwd(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const SceneV
         }
         ws->launches += 2;
     }
+    auto launch_small = [&]() {
+        PhaseTimer timer(ws, DEODR_B200_PH_SMALL_BWD, st);
+        // Triangle-parallel (default) or record-parallel (DEODR_B200_SMALL_ADJOINT=record) adjoint of the small triangles.
+        // In the record-parallel form the vertex gathers and the fifteen atomics per thread are what it costs, not the
+        // bounding-box reads, and more threads pay them; it also slows k_interior_bwd running beside it.
+        if (!ws->small_by_record) {  // (read from the environment when the workspace is created)
+            const int entries = v->hints_exact && !ws->capturing_internally ? plan.hint_small : s.nb_triangles;
+            (tex ? k_small_tri_bwd<MAXC, true> : k_small_tri_bwd<MAXC, false>)<<<at_least_one(grid_for(entries, 128)), 128, 0, st>>>(
+                s, v->tiles_x, v->small_ids.as<int>(), v->scal, edge_cursor, ties, io.owner, image_b, g);
+        } else {
+            const TileSegments seg{v->small_offset.as<int>(), v->small_cursor};
+            (tex ? k_small_rec_bwd<MAXC, true> : k_small_rec_bwd<MAXC, false>)<<<v->num_tiles, 128, 0, st>>>(
+                s, div, seg, v->small_recs.as<PreRec>(), v->scal, edge_cursor, ties, io.owner, image_b, g, maps);
+        }
+        ws->launches++;
+    };
+    bool small_done = false;  // launched before the interior chain when there is one, else after the others
     const bool large = plan.cap_large > 0 && plan.hint_large_tiles > 0;
     if (large) {  // pixels owned by large triangles, tiles without silhouette edges
         cudaStream_t sl = fork_stream(ws, lane, 2, &first);
+        // k_small_tri_bwd is the adjoint's longest kernel.  Launched after k_interior_bwd, its CTAs were dispatched only
+        // once the interior's had taken the SMs, and it ran alone at the end of the step (1M-triangle scene: it began
+        // 54 us into the adjoint).  Launched first (the interior's stream has forked, so it does not wait for it), it
+        // fills the SMs from the start and the interior's CTAs take the slots it leaves.
+        launch_small();
+        small_done = true;
         PhaseTimer timer(ws, DEODR_B200_PH_INTERIOR_BWD, sl);
         const int grid = at_least_one(plan.hint_large_tiles < v->num_tiles ? plan.hint_large_tiles : v->num_tiles);
         (tex ? k_interior_bwd<MAXC, true> : k_interior_bwd<MAXC, false>)<<<grid, NT, 0, sl>>>(
@@ -424,22 +502,7 @@ static void launch_bwd(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const SceneV
                                                        image_b, bg);
         ws->launches++;
     }
-    {
-        PhaseTimer timer(ws, DEODR_B200_PH_SMALL_BWD, st);
-        // Triangle-parallel (default) or record-parallel (DEODR_B200_SMALL_ADJOINT=record) adjoint of the small triangles.
-        // In the record-parallel form the vertex gathers and the fifteen atomics per thread are what it costs, not the
-        // bounding-box reads, and more threads pay them; it also slows k_interior_bwd running beside it.
-        if (!ws->small_by_record) {  // (read from the environment when the workspace is created)
-            const int entries = v->hints_exact && !ws->capturing_internally ? plan.hint_small : s.nb_triangles;
-            (tex ? k_small_tri_bwd<MAXC, true> : k_small_tri_bwd<MAXC, false>)<<<at_least_one(grid_for(entries, 128)), 128, 0, st>>>(
-                s, v->tiles_x, v->small_ids.as<int>(), v->scal, edge_cursor, ties, io.owner, image_b, g);
-        } else {
-            const TileSegments seg{v->small_offset.as<int>(), v->small_cursor};
-            (tex ? k_small_rec_bwd<MAXC, true> : k_small_rec_bwd<MAXC, false>)<<<v->num_tiles, 128, 0, st>>>(
-                s, div, seg, v->small_recs.as<PreRec>(), v->scal, edge_cursor, ties, io.owner, image_b, g, maps);
-        }
-        ws->launches++;
-    }
+    if (!small_done) launch_small();
     if (edges) join_stream(ws, lane, 0);
     if (large) join_stream(ws, lane, 2);
     if (bg_on) join_stream(ws, lane, 1);
@@ -493,3 +556,20 @@ void deodr_launch_backward(DeodrWorkspace *ws, ViewSlot *v, Lane &lane, const Sc
     else if (C <= COLOR_SLAB) launch_bwd<16>(ws, v, lane, s, io, sigma, flags, g, bg);
     else launch_bwd_wide(ws, v, lane, s, io, sigma, flags, g, bg);
 }
+
+#ifdef DEODR_SMALLBWD_PHASE_CLOCKS
+// Measurement builds only: copies k_small_tri_bwd's per-phase cycle sums (SB_PHASES, then the threads and the hidden
+// threads counted) and its owned-pixel histogram (SB_HIST) out of the device, then clears them.  Synchronises the device.
+extern "C" int deodr_b200_small_bwd_phase_clocks(unsigned long long *clocks, unsigned int *hist) {
+    if (cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpyFromSymbol(clocks, g_smallbwd_clocks, sizeof(g_smallbwd_clocks)) != cudaSuccess ||
+        cudaMemcpyFromSymbol(hist, g_smallbwd_hist, sizeof(g_smallbwd_hist)) != cudaSuccess)
+        return DEODR_B200_ECUDA;
+    static const unsigned long long zc[SB_SLOTS] = {};
+    static const unsigned int zh[SB_HIST] = {};
+    if (cudaMemcpyToSymbol(g_smallbwd_clocks, zc, sizeof(zc)) != cudaSuccess ||
+        cudaMemcpyToSymbol(g_smallbwd_hist, zh, sizeof(zh)) != cudaSuccess)
+        return DEODR_B200_ECUDA;
+    return DEODR_B200_OK;
+}
+#endif

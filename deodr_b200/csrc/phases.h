@@ -1023,6 +1023,16 @@ struct AtomicEmit {
     DEODR_HD void emit(float *p, float v) const { Env::atomic_add(p, v); }
 };
 
+// Phases of small_triangle_adjoint, for the cycle counters of a -DDEODR_SMALLBWD_PHASE_CLOCKS build (kernels_bwd.cu
+// defines the hooks there; everywhere else they compile to nothing).
+enum { SB_WALK, SB_EDGE_MASK, SB_SETUP, SB_PIXELS, SB_SCATTER, SB_PHASES };
+#ifndef SMALLBWD_START
+#define SMALLBWD_START ((void)0)
+#define SMALLBWD_LAP(phase) ((void)0)
+#define SMALLBWD_OWNED(mine) ((void)0)
+#define SMALLBWD_DONE ((void)0)
+#endif
+
 // Triangle-parallel interior adjoint of one SMALL triangle (micro-triangle regime): the thread walks the triangle's
 // bounding box, takes the pixels whose adjoint owner it is (the reference's `Z == z_buffer` walk, DR.h:1024, resolved
 // to an owner id by the forward pass), accumulates its vertex gradients in registers and scatters them ONCE: 15
@@ -1032,6 +1042,7 @@ template <int MAXC, class Env>
 DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, const int *edge_tile_count,
                                      const int *owner, const int *tie_pairs, const float *image_b, float *ij_b,
                                      float *colors_b, float *uv_b, float *shade_b, float *texture_b) {
+    SMALLBWD_START;
     const int C = channels<MAXC>(s);
     double V[3][2];
     for (int i = 0; i < 3; i++) {
@@ -1065,7 +1076,12 @@ DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, con
             if (hit) mine |= 1ull << (bit0 + x);
         }
     }
-    if (!mine) return;  // hidden triangle
+    SMALLBWD_LAP(SB_WALK);
+    SMALLBWD_OWNED(mine);
+    if (!mine) {  // hidden triangle
+        SMALLBWD_DONE;
+        return;
+    }
     if (edge_tile_count) {  // pixels of tiles with silhouette edges belong to k_raster_bwd
         for (int ty = y0 / TS; ty <= y1 / TS; ty++)
             for (int tx = x0 / TS; tx <= x1 / TS; tx++) {
@@ -1074,7 +1090,11 @@ DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, con
                     for (int x = (tx * TS > x0 ? tx * TS : x0); x <= x1 && x < (tx + 1) * TS; x++)
                         mine &= ~(1ull << (((y - y0) << shift) + (x - x0)));
             }
-        if (!mine) return;
+        SMALLBWD_LAP(SB_EDGE_MASK);
+        if (!mine) {
+            SMALLBWD_DONE;
+            return;
+        }
     }
     // phase 2: lanes take their i-th owned pixel together; the adjoint colour of the NEXT pixel is loaded while the
     // current one is processed
@@ -1092,6 +1112,7 @@ DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, con
     if (t.textured) {
         VertexGrads<MAXC> acc;
         zero_vertex_grads<MAXC>(s, &acc);
+        SMALLBWD_LAP(SB_SETUP);
         for (;;) {
             const int i = i_next;
             float g[MAXC];
@@ -1106,7 +1127,10 @@ DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, con
             pixel_adjoint<MAXC, Env>(s, t, x0 + (i & stride_mask), y0 + (i >> shift), g, &acc, texture_b);
             if (!more) break;
         }
+        SMALLBWD_LAP(SB_PIXELS);
         flush_vertex_grads<MAXC, AtomicEmit<Env>>(s, t, acc, ij_b, colors_b, uv_b, shade_b, AtomicEmit<Env>());
+        SMALLBWD_LAP(SB_SCATTER);
+        SMALLBWD_DONE;
         return;
     }
     // interpolated triangle: per-triangle constants = vertex colours' screen-space gradient
@@ -1121,6 +1145,7 @@ DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, con
     float gij[3][2] = {{0.0f, 0.0f}, {0.0f, 0.0f}, {0.0f, 0.0f}};
     float gcol[3][MAXC];
     for (int q = 0; q < C; q++) gcol[0][q] = gcol[1][q] = gcol[2][q] = 0.0f;
+    SMALLBWD_LAP(SB_SETUP);
     for (;;) {
         const int i = i_next;
         float g[MAXC];
@@ -1148,11 +1173,14 @@ DEODR_HD void small_triangle_adjoint(const SceneView &s, int k, int tiles_x, con
         gij[2][0] -= w2 * dcdx; gij[2][1] -= w2 * dcdy;
         if (!more) break;
     }
+    SMALLBWD_LAP(SB_PIXELS);
     for (int i = 0; i < 3; i++) {  // same scatter as flush_vertex_grads, interpolated branch
         Env::atomic_add(ij_b + 2 * (size_t)t.vid[i], gij[i][0]);
         Env::atomic_add(ij_b + 2 * (size_t)t.vid[i] + 1, gij[i][1]);
         for (int q = 0; q < C; q++) Env::atomic_add(colors_b + (size_t)t.vid[i] * C + q, gcol[i][q]);
     }
+    SMALLBWD_LAP(SB_SCATTER);
+    SMALLBWD_DONE;
 }
 
 // ---- record-parallel form of the same adjoint -------------------------------------------------------------------
