@@ -255,6 +255,17 @@ class CollisionMesh(C.Structure):
         ("nb_faces", C.c_int32), ("nb_edges", C.c_int32), ("nb_vertices", C.c_int32)]
 
 
+class Skeleton(C.Structure):
+    """``DeodrSkeleton``: the device arrays of the linear blend skinning entry points."""
+
+    _fields_ = [(name, C.c_void_p) for name in ("parents", "centres", "level_offset", "level_index", "child_offset",
+                                                 "child_index", "skin_index", "skin_weight", "joint_offset",
+                                                 "joint_entry", "chunk_offset")] + [
+        (name, C.c_int32) for name in ("nb_joints", "nb_vertices", "nb_influences", "nb_levels", "nb_chunks", "pad")]
+
+
+SKIN_MAX_JOINTS, SKIN_MAX_INFLUENCES, SKIN_CHUNK = 1024, 8, 256  # the header's DEODR_B200_SKIN_* values
+
 # every symbol include/deodr_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("deodr_b200_workspace_create", C.c_int, [C.POINTER(C.c_void_p), C.c_int]),
@@ -421,6 +432,9 @@ SYMBOLS = [
     ("deodr_b200_self_intersections", C.c_int,
      [C.c_void_p, C.POINTER(CollisionMesh), C.c_void_p, C.c_double, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
       C.c_void_p]),
+    ("deodr_b200_skin", C.c_int, [C.POINTER(Skeleton), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("deodr_b200_skin_b", C.c_int,
+     [C.POINTER(Skeleton)] + [C.c_void_p] * 10),
     ("deodr_b200_render_host", C.c_int,
      [C.c_void_p, C.POINTER(HostScene), C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p]),
     ("deodr_b200_render_b_host", C.c_int,

@@ -9,6 +9,11 @@ the kernels of csrc/fitter.cu (include/deodr_b200.h, "mesh fitting").  Nothing i
 ``step()`` apart from the renderer's own verdict (and, with ``cself > 0``, the self-collision's); its energy is a 0-d
 fp64 CUDA tensor.  With ``cself > 0`` the step adds ``DeviceSelfCollisionEnergy`` of the un-posed vertices to the
 rigidity's gradient and energy; ``energy_self_collision`` holds its energy.
+
+``MeshDepthFitter`` and ``MeshRGBFitterWithPose`` also take ``skeleton``: a ``LinearBlendSkinning`` (or its four
+arrays), whose joint rotations [J,3] are fitted with the rest.  The step then skins the vertices before the rigid pose,
+evaluates the self-collision at the skinned vertices (where joints bend, distances change), back-propagates through the
+skinning to the rest vertices and the rotations, and keeps the Laplacian rigidity on the rest vertices.
 """
 
 from __future__ import annotations
@@ -21,8 +26,8 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .mesh_ops import (CameraParams, DeviceMeshView, MeshTopology, _f64, _stream, project_points,
-                       project_points_backward, topology_arrays)
+from .mesh_ops import (CameraParams, DeviceMeshView, LinearBlendSkinning, MeshTopology, _f64, _stream,
+                       project_points, project_points_backward, topology_arrays)
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -334,18 +339,30 @@ def fitter_camera(camera_center, width: int, height: int, focal=None, distortion
     return CameraParams(np.column_stack((rot, trans)), intrinsic, distortion)
 
 
+# The heavy-ball step of the joint rotations (radians).  On the articulated-fit tube of tests/test_gpu_skinning.py
+# (128 x 128 colour image, bends of 0.3 - 0.4 rad) the joint gradients start near 3e3, so the step runs at its clamp
+# at first; 0.05 rad (about 3 degrees) per step bounds it.  Measured on an H100 over 800 steps: with the per-vertex
+# deformation held still, 0.002 recovers the bends within 0.046 rad in 16 runs out of 16 (0.0005 within 0.015); with
+# it free, 0.0005 leaves the joints nearly where they start, since the vertices take the bend, and of 0.002, 0.005,
+# 0.02 and 0.05, 0.002 ends closest.  The free deformation then absorbs part of the bend whatever the factor.
+STEP_FACTOR_JOINTS = 0.002
+STEP_MAX_JOINTS = 0.05
+
+
 class _PoseFitter:
     """State and update rule shared by the two fitters: vertices, quaternion and translation with their speeds."""
 
     def _init_pose(self, vertices, faces, euler_init, translation_init, cregu, inertia, damping, device, cself=0.0,
-                   self_collision_thickness=None):
+                   self_collision_thickness=None, skeleton=None):
         self.device = torch.device(device)
         self.cregu, self.inertia, self.damping = cregu, inertia, damping
         self.faces = np.ascontiguousarray(np.asarray(faces), dtype=np.int64)
         self.vertices_init = np.array(vertices, dtype=np.float64)
         self.nb_vertices = self.vertices_init.shape[0]
         self.rigid_energy = DeviceLaplacianRigidEnergy(self.faces, self.vertices_init, cregu, self.device)
-        # the self-collision term, evaluated at the un-posed vertices (the pose is rigid: distances do not change)
+        self.skinning = self._skinning(skeleton)
+        # the self-collision term, evaluated at the vertices the rigid pose moves (the pose is rigid: distances do not
+        # change under it), i.e. the skinned vertices with a skeleton
         self.cself = float(cself)
         self.self_collision = None
         self.energy_self_collision = torch.zeros((), dtype=torch.float64, device=self.device)
@@ -359,6 +376,33 @@ class _PoseFitter:
         self._scratch = new_scratch(self.device)
         self.view: Optional[DeviceMeshView] = None
         self.set_mesh_transform_init(euler=euler_init, translation=translation_init)
+
+    def _skinning(self, skeleton) -> Optional[LinearBlendSkinning]:
+        """The skeleton of the articulated fit, or None.  A single root at joint 0 is required: its rotation would
+        duplicate the rigid quaternion, so it stays fixed and rows 1..J-1 of ``joint_rotations`` are fitted."""
+        if skeleton is None:
+            return None
+        if not isinstance(skeleton, LinearBlendSkinning):
+            skeleton = LinearBlendSkinning(*skeleton, device=self.device)
+        device = self.rigid_energy.vertices_ref.device
+        if skeleton.device != device or skeleton.nb_vertices != self.nb_vertices:
+            raise ValueError(f"the skeleton binds {skeleton.nb_vertices} vertices on {skeleton.device}; the mesh has "
+                             f"{self.nb_vertices} on {device}")
+        roots = np.flatnonzero(skeleton.parents < 0)
+        if roots.tolist() != [0]:
+            raise ValueError("the fitters need a skeleton with a single root at joint 0; "
+                             f"its roots are {roots.tolist()}")
+        self.joint_rotations_init = np.zeros((skeleton.nb_joints, 3))
+        return skeleton
+
+    def set_joint_rotations_init(self, rotations) -> None:
+        """The joint rotations [J,3] (axis-angle) that :meth:`reset` starts from; row 0, the root's, stays fixed."""
+        if self.skinning is None:
+            raise ValueError("set_joint_rotations_init needs a fitter built with a skeleton")
+        rotations = np.array(rotations, dtype=np.float64)
+        if rotations.shape != (self.skinning.nb_joints, 3) or not np.all(np.isfinite(rotations)):
+            raise ValueError(f"rotations must be finite [{self.skinning.nb_joints},3]; got shape {rotations.shape}")
+        self.joint_rotations_init = rotations
 
     def _tensor(self, a) -> torch.Tensor:
         return torch.tensor(np.array(a, dtype=np.float64), device=self.device)
@@ -382,6 +426,12 @@ class _PoseFitter:
         self.transform_translation_b = torch.empty(3, dtype=torch.float64, device=dev)
         self._grad_rigid = torch.empty((V, 3), dtype=torch.float64, device=dev)
         self._energy_rigid = torch.empty((), dtype=torch.float64, device=dev)
+        if self.skinning is not None:
+            self.joint_rotations = self._tensor(self.joint_rotations_init)
+            self.speed_joint_rotations = torch.zeros_like(self.joint_rotations)
+            self.joint_rotations_b = torch.empty_like(self.joint_rotations)
+            self._skinned = torch.empty((V, 3), dtype=torch.float64, device=dev)
+            self._skinned_b = torch.empty((V, 3), dtype=torch.float64, device=dev)
         self.iter = 0
 
     def _camera(self, mesh_image, focal, distortion) -> CameraParams:
@@ -399,19 +449,42 @@ class _PoseFitter:
             self._energy_rigid += self.energy_self_collision
 
     def _render_pose(self) -> torch.Tensor:
-        return pose(self.vertices, self.transform_quaternion, self.transform_translation, self._scratch,
+        vertices = self.vertices
+        if self.skinning is not None:
+            vertices = self.skinning.apply(self.vertices, self.joint_rotations, out=self._skinned)
+        return pose(vertices, self.transform_quaternion, self.transform_translation, self._scratch,
                     out=self._transformed)
+
+    def _skinning_backward(self, transformed_b: torch.Tensor) -> None:
+        """The articulated step's adjoint: the pose's to the (centred) skinned vertices, plus the self-collision's
+        there, then the skinning's to the rest vertices and the joint rotations; the rigidity on the rest vertices."""
+        pose_backward(self._skinned, self.transform_quaternion, transformed_b, self._scratch,
+                      out=(self._skinned_b, self.transform_quaternion_b, self.transform_translation_b))
+        if self.self_collision is not None:
+            self.self_collision.evaluate(self._skinned, grad=self._skinned_b, energy=self.energy_self_collision,
+                                         add_to=self._skinned_b)
+        self.skinning.backward(self.vertices, self.joint_rotations, self._skinned_b,
+                               out=(self._vertices_b, self.joint_rotations_b))
+        self.rigid_energy.evaluate(self.vertices, grad=self._grad_rigid, energy=self._energy_rigid)
+        if self.self_collision is not None:
+            self._energy_rigid += self.energy_self_collision
 
     def _pose_backward_rigid_update(self, transformed_b: torch.Tensor, energy_data: torch.Tensor,
                                     extra_params=()) -> torch.Tensor:
-        pose_backward(self.vertices, self.transform_quaternion, transformed_b, self._scratch,
-                      out=(self._vertices_b, self.transform_quaternion_b, self.transform_translation_b))
-        self._regularisers()
+        if self.skinning is None:
+            pose_backward(self.vertices, self.transform_quaternion, transformed_b, self._scratch,
+                          out=(self._vertices_b, self.transform_quaternion_b, self.transform_translation_b))
+            self._regularisers()
+        else:
+            self._skinning_backward(transformed_b)
         energy = torch.empty((), dtype=torch.float64, device=self.device)
         params = [heavy_ball(self.transform_quaternion, self.speed_quaternion, self.transform_quaternion_b,
                              self.step_factor_quaternion, self.step_max_quaternion, normalize=True),
                   heavy_ball(self.transform_translation, self.speed_translation, self.transform_translation_b,
                              self.step_factor_translation, self.step_max_translation)] + list(extra_params)
+        if self.skinning is not None and self.skinning.nb_joints > 1:  # rows 1..J-1: the root stays fixed
+            params.append(heavy_ball(self.joint_rotations[1:], self.speed_joint_rotations[1:],
+                                     self.joint_rotations_b[1:], self.step_factor_joints, self.step_max_joints))
         fitter_update(heavy_ball(self.vertices, self.speed_vertices, self._vertices_b, self.step_factor_vertices,
                                  self.step_max_vertices), self._grad_rigid, params, self.inertia, self.damping,
                       energy_data, self._energy_rigid, energy, self.device)
@@ -425,13 +498,14 @@ class MeshDepthFitter(_PoseFitter):
 
     def __init__(self, vertices, faces, euler_init, translation_init, cregu: float = 2000, inertia: float = 0.96,
                  damping: float = 0.05, device="cuda", cself: float = 0.0,
-                 self_collision_thickness: Optional[float] = None):
+                 self_collision_thickness: Optional[float] = None, skeleton=None):
         self.step_factor_vertices = 0.0005
         self.step_max_vertices = 1
         self.step_factor_quaternion = 0.00006
         self.step_max_quaternion = 0.1
         self.step_factor_translation = 0.00005
         self.step_max_translation = 0.1
+        self.step_factor_joints, self.step_max_joints = STEP_FACTOR_JOINTS, STEP_MAX_JOINTS
         vertices = np.asarray(vertices, dtype=np.float64)
         object_center = vertices.mean(axis=0)
         object_radius = np.max(np.std(vertices, axis=0))
@@ -439,7 +513,7 @@ class MeshDepthFitter(_PoseFitter):
         self.max_depth = None
         self.depth_scale = 1.0
         self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device, cself,
-                        self_collision_thickness)
+                        self_collision_thickness, skeleton)
         self.reset()
 
     def reset(self) -> None:
@@ -485,13 +559,14 @@ class MeshRGBFitterWithPose(_PoseFitter):
     def __init__(self, vertices, faces, euler_init, translation_init, default_color, default_light_directional,
                  default_light_ambient: float, cregu: float = 2000, inertia: float = 0.96, damping: float = 0.05,
                  update_lights: bool = True, update_color: bool = True, device="cuda",
-                 cself: float = 0.0, self_collision_thickness: Optional[float] = None):
+                 cself: float = 0.0, self_collision_thickness: Optional[float] = None, skeleton=None):
         self.step_factor_vertices = 0.0005
         self.step_max_vertices = 0.5
         self.step_factor_quaternion = 0.00006
         self.step_max_quaternion = 0.05
         self.step_factor_translation = 0.00005
         self.step_max_translation = 0.1
+        self.step_factor_joints, self.step_max_joints = STEP_FACTOR_JOINTS, STEP_MAX_JOINTS
         self.default_color = np.array(default_color, dtype=np.float64)
         self.default_light_directional = np.array(default_light_directional, dtype=np.float64)
         self.default_light_ambient = float(default_light_ambient)
@@ -504,7 +579,7 @@ class MeshRGBFitterWithPose(_PoseFitter):
         self.background_color = None
         self.sigma = 1.0
         self._init_pose(vertices, faces, euler_init, translation_init, cregu, inertia, damping, device, cself,
-                        self_collision_thickness)
+                        self_collision_thickness, skeleton)
         self.reset()
 
     def reset(self) -> None:

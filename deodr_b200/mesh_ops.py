@@ -1306,6 +1306,159 @@ def loop_subdivision(faces, vertices, colors=None, n_iter: int = 1):
     return sub.faces, fv.cpu().numpy(), (fc.cpu().numpy() if fc is not None else None)
 
 
+def skeleton_arrays(parents, joints, skin_index, skin_weight) -> dict:
+    """Host arrays of ``DeodrSkeleton`` (include/deodr_b200.h, "Linear blend skinning"), built and checked here:
+    ``parents`` [J] (parents[j] < j, -1 for a root), ``joints`` [J,3] rest centres, ``skin_index`` [V,K] joints in
+    [0, J) and ``skin_weight`` [V,K] (not renormalised), 1 <= J <= 1024 and 1 <= K <= 8.  Adds the depth levels (the
+    roots first), the children CSR and the joint CSR of the entries i*K+k (ascending in every row), cut in chunks of
+    ``SKIN_CHUNK`` entries.  Raises ValueError for a parent that is not lower than its joint, an index outside
+    [0, J), a non-finite centre or weight, or a J, V or K out of range."""
+    parents = np.asarray(parents)
+    joints = np.asarray(joints, dtype=np.float64)
+    skin_index = np.asarray(skin_index)
+    skin_weight = np.asarray(skin_weight, dtype=np.float64)
+    if parents.ndim != 1 or not 1 <= parents.size <= _cabi.SKIN_MAX_JOINTS:
+        raise ValueError(f"parents must be [J] with 1 <= J <= {_cabi.SKIN_MAX_JOINTS}; got shape {parents.shape}")
+    J = parents.size
+    if not np.issubdtype(parents.dtype, np.integer) or not np.issubdtype(skin_index.dtype, np.integer):
+        raise ValueError("parents and skin_index must be integer arrays")
+    parents = parents.astype(np.int64)
+    if np.any(parents >= np.arange(J)):
+        raise ValueError("every parent must be lower than its joint (parents[j] < j)")
+    if np.any(parents < -1):
+        raise ValueError("a parent must be a joint index in [0, J) or -1 for a root")
+    if joints.shape != (J, 3):
+        raise ValueError(f"joints must be [{J},3]; got {joints.shape}")
+    if skin_index.ndim != 2 or skin_index.shape[0] < 1 or not 1 <= skin_index.shape[1] <= _cabi.SKIN_MAX_INFLUENCES:
+        raise ValueError(f"skin_index must be [V,K] with V >= 1 and 1 <= K <= {_cabi.SKIN_MAX_INFLUENCES}; "
+                         f"got shape {skin_index.shape}")
+    if skin_weight.shape != skin_index.shape:
+        raise ValueError(f"skin_weight must be {skin_index.shape} like skin_index; got {skin_weight.shape}")
+    V, K = skin_index.shape
+    if V * K > 0x7FFFFFFF:
+        raise ValueError("V * K must fit in int32")
+    if np.any(skin_index < 0) or np.any(skin_index >= J):
+        raise ValueError(f"skin_index must lie in [0, {J})")
+    if not np.all(np.isfinite(joints)) or not np.all(np.isfinite(skin_weight)):
+        raise ValueError("joint centres and skinning weights must be finite")
+    depth = np.zeros(J, dtype=np.int64)
+    for j in range(J):
+        if parents[j] >= 0:
+            depth[j] = depth[parents[j]] + 1
+    nb_levels = int(depth.max()) + 1
+
+    def csr(rows, n):
+        offset = np.zeros(n + 1, dtype=np.int32)
+        np.cumsum(np.bincount(rows, minlength=n), out=offset[1:])
+        return offset, np.argsort(rows, kind="stable").astype(np.int32)
+
+    level_offset, level_index = csr(depth, nb_levels)
+    non_roots = np.flatnonzero(parents >= 0)
+    child_offset = np.zeros(J + 1, dtype=np.int32)
+    np.cumsum(np.bincount(parents[non_roots], minlength=J), out=child_offset[1:])
+    child_index = non_roots[np.argsort(parents[non_roots], kind="stable")].astype(np.int32)
+    joint_offset, joint_entry = csr(skin_index.reshape(-1).astype(np.int64), J)
+    chunks = (np.diff(joint_offset) + _cabi.SKIN_CHUNK - 1) // _cabi.SKIN_CHUNK
+    chunk_offset = np.zeros(J + 1, dtype=np.int32)
+    np.cumsum(chunks, out=chunk_offset[1:])
+    return {"parents": parents.astype(np.int32), "centres": np.ascontiguousarray(joints),
+            "level_offset": level_offset, "level_index": level_index, "child_offset": child_offset,
+            "child_index": child_index if child_index.size else np.zeros(1, np.int32),
+            "skin_index": np.ascontiguousarray(skin_index, dtype=np.int32),
+            "skin_weight": np.ascontiguousarray(skin_weight), "joint_offset": joint_offset, "joint_entry": joint_entry,
+            "chunk_offset": chunk_offset, "nb_joints": J, "nb_vertices": V, "nb_influences": K,
+            "nb_levels": nb_levels, "nb_chunks": int(chunk_offset[-1])}
+
+
+class LinearBlendSkinning:
+    """A mesh articulated by a skeleton (include/deodr_b200.h, "Linear blend skinning"), on the device: the host
+    arrays of :func:`skeleton_arrays` are built and uploaded once, then :meth:`apply` maps rest vertices [V,3] and
+    axis-angle joint rotations [J,3] to skinned vertices, and :meth:`backward` maps their gradient back to the rest
+    vertices, the rotations and, on request, the weights.  Neither synchronises with the host; the adjoint uses no
+    atomics, so it gives the same bits from call to call.  The joint centres are constants.
+
+    ``transforms`` [J,24] is the forward kinematics table (Rg, tg, M, b per joint) that :meth:`apply` writes and
+    :meth:`backward` re-reads: both use the binding's own table unless given one, so a backward belongs to the last
+    apply unless the two share a table.  ``skin_weight`` [V,K] replaces the bound weights in a call (the joint CSR
+    depends on the indices only)."""
+
+    def __init__(self, parents, joints, skin_index, skin_weight, device="cuda"):
+        self.device = torch.device(device)
+        arrays = skeleton_arrays(parents, joints, skin_index, skin_weight)
+        self.parents = arrays["parents"]
+        self.nb_joints, self.nb_vertices, self.nb_influences = (arrays["nb_joints"], arrays["nb_vertices"],
+                                                                arrays["nb_influences"])
+        self.nb_chunks = arrays["nb_chunks"]
+        self.t = {k: torch.from_numpy(v).to(self.device) for k, v in arrays.items() if isinstance(v, np.ndarray)}
+        self.device = self.t["parents"].device  # "cuda" -> "cuda:N", as the tensors of the calls report it
+        self.skin_weight = self.t["skin_weight"]
+        self._struct = _cabi.Skeleton()
+        for name, t in self.t.items():
+            setattr(self._struct, name, t.data_ptr())
+        for name in ("nb_joints", "nb_vertices", "nb_influences", "nb_levels", "nb_chunks"):
+            setattr(self._struct, name, arrays[name])
+        self.transforms = torch.zeros((self.nb_joints, 24), dtype=torch.float64, device=self.device)
+        self._scratch = torch.empty(((self.nb_chunks + self.nb_joints) * 12,), dtype=torch.float64, device=self.device)
+
+    def _check(self, x: torch.Tensor, shape: Tuple[int, int], name: str) -> torch.Tensor:
+        if tuple(x.shape) != shape:
+            raise ValueError(f"{name} must be {list(shape)}; got {tuple(x.shape)}")
+        return _f64(x, self.device)
+
+    def _skeleton(self, skin_weight: Optional[torch.Tensor]) -> Tuple[_cabi.Skeleton, Optional[torch.Tensor]]:
+        if skin_weight is None:
+            return self._struct, None
+        w = self._check(skin_weight, (self.nb_vertices, self.nb_influences), "skin_weight")
+        s = _cabi.Skeleton.from_buffer_copy(self._struct)
+        s.skin_weight = w.data_ptr()
+        return s, w
+
+    def _table(self, transforms: Optional[torch.Tensor]) -> torch.Tensor:
+        if transforms is None:
+            return self.transforms
+        if tuple(transforms.shape) != (self.nb_joints, 24) or transforms.dtype != torch.float64 or \
+                transforms.device != self.device or not transforms.is_contiguous():
+            raise ValueError(f"transforms must be a contiguous [{self.nb_joints},24] fp64 tensor on {self.device}")
+        return transforms
+
+    def apply(self, vertices: torch.Tensor, rotations: torch.Tensor, skin_weight: Optional[torch.Tensor] = None,
+              transforms: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """rest vertices [V,3] and rotations [J,3] -> skinned vertices [V,3] fp64 (into ``out`` when given)."""
+        v = self._check(vertices, (self.nb_vertices, 3), "vertices")
+        r = self._check(rotations, (self.nb_joints, 3), "rotations")
+        s, w = self._skeleton(skin_weight)
+        table = self._table(transforms)
+        if out is None:
+            out = torch.empty((self.nb_vertices, 3), dtype=torch.float64, device=self.device)
+        _cabi.check(_cabi.load().deodr_b200_skin(C.byref(s), v.data_ptr(), r.data_ptr(), table.data_ptr(),
+                                                 out.data_ptr(), _stream(self.device)))
+        return out
+
+    def backward(self, vertices: torch.Tensor, rotations: torch.Tensor, skinned_b: torch.Tensor,
+                 weights_grad: bool = False, skin_weight: Optional[torch.Tensor] = None,
+                 transforms: Optional[torch.Tensor] = None, add_to: Optional[torch.Tensor] = None, out=None):
+        """-> (vertices_b [V,3], rotations_b [J,3]) or, with ``weights_grad``, (vertices_b, rotations_b, weights_b
+        [V,K]), fp64, from skinned_b [V,3].  vertices_b = add_to + the adjoint (``add_to`` may be ``vertices_b``
+        itself).  ``out`` = (vertices_b, rotations_b) buffers to write into."""
+        v = self._check(vertices, (self.nb_vertices, 3), "vertices")
+        r = self._check(rotations, (self.nb_joints, 3), "rotations")
+        g = self._check(skinned_b, (self.nb_vertices, 3), "skinned_b")
+        s, w = self._skeleton(skin_weight)
+        table = self._table(transforms)
+        if out is None:
+            out = (torch.empty((self.nb_vertices, 3), dtype=torch.float64, device=self.device),
+                   torch.empty((self.nb_joints, 3), dtype=torch.float64, device=self.device))
+        v_b, r_b = out
+        w_b = (torch.empty((self.nb_vertices, self.nb_influences), dtype=torch.float64, device=self.device)
+               if weights_grad else None)
+        _cabi.check(_cabi.load().deodr_b200_skin_b(
+            C.byref(s), v.data_ptr(), r.data_ptr(), table.data_ptr(), g.data_ptr(),
+            add_to.data_ptr() if add_to is not None else None, v_b.data_ptr(),
+            w_b.data_ptr() if w_b is not None else None, r_b.data_ptr(), self._scratch.data_ptr(),
+            _stream(self.device)))
+        return (v_b, r_b, w_b) if weights_grad else (v_b, r_b)
+
+
 SHADOW_MAP_SIZES = (8, 4096)
 
 

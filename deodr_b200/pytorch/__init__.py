@@ -19,6 +19,7 @@ from .scene3d_pytorch import (  # noqa: F401
     CameraPytorch,
     ColoredTriMeshPytorch,
     LaplacianRigidEnergyPytorch,
+    LinearBlendSkinningFunc,
     LitVertexColorsFunc,
     LoopSubdivisionFunc,
     PhongShadeFunc,

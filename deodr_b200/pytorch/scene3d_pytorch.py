@@ -70,7 +70,8 @@ import numpy as np
 import torch
 
 from ..mesh_fitter import DeviceLaplacianRigidEnergy, DeviceSelfCollisionEnergy, new_scratch, pose, pose_backward
-from ..mesh_ops import (CameraParams, LoopSubdivision, MeshTopology, camera_center, lit_vertex_colors,
+from ..mesh_ops import (CameraParams, LinearBlendSkinning, LoopSubdivision, MeshTopology, camera_center,
+                        lit_vertex_colors,
                         ShadowCubes, SunShadowMap, check_shadow_arguments, check_sun_shadow_arguments,
                         cube_project_backward, lit_vertex_colors_backward, sun_project_backward, sun_visibility,
                         sun_visibility_backward,
@@ -494,6 +495,33 @@ class LoopSubdivisionFunc(torch.autograd.Function):
         gv, gc = ctx.sub.backward(vb, cb)
         vd, cd = ctx.dtypes
         return (gv.to(vd) if gv is not None else None), (gc.to(cd) if gc is not None else None), None
+
+
+class LinearBlendSkinningFunc(torch.autograd.Function):
+    """Linear blend skinning: (vertices [V,3], rotations [J,3] axis-angle, skin_weight [V,K], LinearBlendSkinning) ->
+    skinned vertices [V,3], fp64 (deodr_b200_skin).  The forward kinematics table is the node's own, so forwards may
+    run in any order before their backwards; backward (deodr_b200_skin_b, bit-reproducible) returns the gradients of
+    the vertices and the rotations, and of the weights when they require it.  The joint centres are constants."""
+
+    @staticmethod
+    def forward(ctx: Any, vertices: torch.Tensor, rotations: torch.Tensor, skin_weight: torch.Tensor,  # type: ignore
+                skinning: LinearBlendSkinning):
+        v, r, w = _f64(vertices), _f64(rotations), _f64(skin_weight)
+        table = torch.empty((skinning.nb_joints, 24), dtype=torch.float64, device=skinning.device)
+        out = skinning.apply(v, r, skin_weight=w, transforms=table)
+        ctx.save_for_backward(v, r, w, table)
+        ctx.skinning = skinning
+        ctx.dtypes = (vertices.dtype, rotations.dtype, skin_weight.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx: Any, skinned_b: torch.Tensor):  # type: ignore
+        v, r, w, table = ctx.saved_tensors
+        need_w = ctx.needs_input_grad[2]
+        res = ctx.skinning.backward(v, r, skinned_b.to(torch.float64).contiguous(), weights_grad=need_w,
+                                    skin_weight=w, transforms=table)
+        vd, rd, wd = ctx.dtypes
+        return res[0].to(vd), res[1].to(rd), (res[2].to(wd) if need_w else None), None
 
 
 class PhongShadeFunc(torch.autograd.Function):

@@ -1116,6 +1116,62 @@ int deodr_b200_self_collision(DeodrWorkspace *ws, const DeodrCollisionMesh *mesh
 int deodr_b200_self_intersections(DeodrWorkspace *ws, const DeodrCollisionMesh *mesh, const double *vertices,
                                   double cell_size, int32_t *pairs, int64_t capacity, int64_t *count, void *stream);
 
+/* ---- Linear blend skinning: a mesh articulated by a skeleton, and its adjoint, in fp64 on device buffers
+ * (csrc/skinning.cu).  A skeleton has J joints; joint j has a parent parents[j] < j, or -1 for a root (several roots
+ * are allowed), and a rest centre c_j [3].  Vertex i has K influences: joints skin_index[i,k] in [0, J) with weights
+ * skin_weight[i,k].  Weights are not renormalised: identity rotations leave a vertex at rest only when its weights
+ * sum to 1 (this is not checked).
+ *   R(theta) = I + a [theta]x + b [theta]x^2,  phi = |theta|,  a = sin(phi) / phi,  b = (1 - cos(phi)) / phi^2
+ *              (the axis-angle of MANO / SMPL; below phi = 0.1 the series of a, b and their derivatives, so R and
+ *              dR/dtheta are exact and finite at theta = 0, where dR/dtheta_k = [e_k]x)
+ *   forward kinematics, in index order:  root: Rg_j = R(theta_j), tg_j = c_j;
+ *                                        else: Rg_j = Rg_p R(theta_j), tg_j = tg_p + Rg_p (c_j - c_p)
+ *   skinning transforms:  M_j = Rg_j,  b_j = tg_j - Rg_j c_j      (identity rotations give (I, 0))
+ *   skinned vertices:     v'_i = sum_k w_ik (M_j v_i + b_j),  j = skin_index[i,k]
+ * Adjoint, from g = dL/dv' [V,3]:
+ *   vertices_b_i  = sum_k w_ik M_j^T g_i
+ *   weights_b_ik  = g_i . (M_j v_i + b_j)
+ *   rotations_b   [J,3]: (M_b, b_b)_j = sum over the influences on j of (w g v^T, w g), back through the forward
+ *                 kinematics.  The joint centres get no gradient.
+ * The host builds the index arrays and checks their contents (deodr_b200.mesh_ops.skeleton_arrays); the calls check
+ * sizes and pointers only. */
+enum {
+    DEODR_B200_SKIN_MAX_JOINTS = 1024,   /* the forward kinematics run in one CTA, one thread per joint of a level */
+    DEODR_B200_SKIN_MAX_INFLUENCES = 8,  /* as glTF's JOINTS_n / WEIGHTS_n */
+    DEODR_B200_SKIN_CHUNK = 256          /* entries of a joint's CSR row summed by one CTA of the adjoint */
+};
+typedef struct DeodrSkeleton {
+    const int32_t *parents;       /* [J] */
+    const double *centres;        /* [J,3] rest centres */
+    const int32_t *level_offset;  /* [nb_levels+1] CSR: the joints of every depth (the roots are depth 0) ... */
+    const int32_t *level_index;   /* ... [J], ascending in every level */
+    const int32_t *child_offset;  /* [J+1] CSR: the children of every joint ... */
+    const int32_t *child_index;   /* ... ascending (J minus the roots entries; required even when empty) */
+    const int32_t *skin_index;    /* [V,K] */
+    const double *skin_weight;    /* [V,K] */
+    const int32_t *joint_offset;  /* [J+1] CSR: the influences i*K+k on every joint ... */
+    const int32_t *joint_entry;   /* ... [V*K], ascending in every row */
+    const int32_t *chunk_offset;  /* [J+1] the first chunk of every joint: row j has ceil(n_j / SKIN_CHUNK) chunks */
+    int32_t nb_joints, nb_vertices, nb_influences, nb_levels, nb_chunks, pad;
+} DeodrSkeleton;
+
+/* skinned [V,3] from vertices [V,3] and rotations [J,3]: one single-CTA launch of the forward kinematics, a barrier per
+ * depth level, which writes transforms [J,24] = (Rg [9], tg [3], M [9], b [3]) per joint, then one thread per vertex.
+ * EINVAL before any launch for a NULL skeleton, skeleton array or argument, J outside [1, 1024], V < 1, K outside
+ * [1, 8] or nb_levels outside [1, J]; EUNSUPPORTED when V * K does not fit in int32.  No host synchronisation. */
+int deodr_b200_skin(const DeodrSkeleton *skeleton, const double *vertices, const double *rotations, double *transforms,
+                    double *skinned, void *stream);
+/* The adjoint of deodr_b200_skin from skinned_b [V,3], re-reading the transforms [J,24] the forward wrote for the same
+ * rotations: vertices_b [V,3] = grad_in + sum_k w_ik M_j^T g_i (grad_in may be NULL, or equal to vertices_b to add in
+ * place), weights_b [V,K] when not NULL, and rotations_b [J,3] (overwritten).  scratch holds (nb_chunks + J) * 12
+ * doubles.  Three launches: one thread per vertex; one CTA per chunk of a joint's CSR row, summed in a fixed order;
+ * one CTA that adds every joint's chunks in chunk order and walks the levels back, each parent gathering its children
+ * in children-CSR order.  No fp64 atomics: two calls on the same input give the same bits.  Refusals as above, with
+ * a NULL skinned_b, vertices_b, rotations_b or scratch.  No host synchronisation. */
+int deodr_b200_skin_b(const DeodrSkeleton *skeleton, const double *vertices, const double *rotations,
+                      const double *transforms, const double *skinned_b, const double *grad_in, double *vertices_b,
+                      double *weights_b, double *rotations_b, double *scratch, void *stream);
+
 /* Per-kernel device timing with CUDA events recorded on the launching stream (for bench.py's roofline).
  * enable: pre-creates `max_records` event pairs (0 disables and frees them).  Every instrumented launch group of the
  * following render / render_b calls then records one (phase, start, stop) triple until the pool is exhausted.
